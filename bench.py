@@ -56,18 +56,20 @@ def parse():
     ap.add_argument("--cpu-sample", type=int, default=16, help="targets in the CPU baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--seed", type=int, default=1)
-    ap.add_argument("--feature-threads", type=int, default=8, help="reference -t: host threads submitting targets (4 threads stage ~40 targets/ms, about what one B200 consumes)")
+    ap.add_argument("--feature-threads", type=int, default=8, help="reference -t: host threads submitting targets")
     ap.add_argument("--e2e-launch-targets", type=int, default=2000, help="hb_options.launch_targets in the e2e regions (shared by the feature "
                     "threads: each hands over max(256, launch_targets / threads) targets per device launch; measured on cfg3 with 8 threads: "
                     "256-target launches 800-868 Mbases/s, 500: 785-796, 1000: 709, 2000: 584 - smaller launches overlap better across the lanes)")
     ap.add_argument("--host-windowing", action="store_true", help="e2e region submits host-computed OverlapWindows (hb_submit_target) instead of raw alignments")
     ap.add_argument("--cpu-threads", type=int, default=0, help="threads of the CPU legs (cpu_baseline / --impl reference); 0 = all host threads")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the corrected reads of a fixed sample of the last timed step's targets as DIR/*.npy")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """SM clocks / throttle reasons of the job's GPUs DURING the timed region (B200_PROFILING.md).  One sampler for the whole
+    """SM clocks / throttle reasons of the job's GPUs DURING the timed region.  One sampler for the whole
     job (rank 0), through NVML in-process: a poller per rank spawning nvidia-smi five times a second contends for the driver
     with the very launches being timed (measured at N=4).  Falls back to nvidia-smi when pynvml is unavailable."""
 
@@ -222,13 +224,43 @@ def workload_name(args):
 
 
 def ensure_model():
+    # a temporary file: the benchmark writes nothing into the source tree (it may be read-only)
+    import tempfile
     from herro_b200 import weights as hbw
-    d = os.path.join(ROOT, "tests", "_tmp")
-    os.makedirs(d, exist_ok=True)
-    p = os.path.join(d, f"bench_model_{os.getpid()}.hbw")
+    p = os.path.join(tempfile.gettempdir(), f"herro_bench_model_{os.getpid()}.hbw")
     cfg = hbw.NetConfig()
     hbw.save_blob(p, cfg, hbw.random_weights(cfg, seed=7))
     return p, cfg
+
+
+DUMP_TARGETS = 256          # targets in the --dump-outputs sample
+DUMP_MAX_BASES = 14 << 20   # float32 bases kept in the dump (56 MB; the segment tables stay far below the 64 MB budget)
+
+
+def dump_outputs(ctx, harness, t_begin, t_end, out_dir):
+    """Corrected reads of a fixed, seeded sample of targets [t_begin, t_end) (the last timed step), resubmitted through the
+    same context, as a caller of hb_submit_alignments / hb_poll_corrected receives them: per segment its target id, index
+    and length, and the concatenated bases as float32 ASCII codes."""
+    rng = np.random.default_rng(12345)
+    pick = np.sort(rng.choice(np.arange(t_begin, t_end), size=min(DUMP_TARGETS, t_end - t_begin), replace=False))
+    for t in pick:
+        a, b = int(harness.aln_off[t]), int(harness.aln_off[t + 1])
+        if b > a:
+            ctx.submit_alignments(int(t), harness.ovl[a:b])
+    ctx.flush()
+    rid, idx, lens, bases, n = [], [], [], [], 0
+    for r in sorted(ctx.drain(skip_failed=True), key=lambda r: r.rid):
+        if n + sum(len(x) for x in r.segments) > DUMP_MAX_BASES:
+            break
+        for k, seg in enumerate(r.segments):
+            rid.append(r.rid); idx.append(k); lens.append(len(seg)); bases.append(np.frombuffer(seg, np.uint8))
+            n += len(seg)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sampled_targets.npy"), pick.astype(np.float64))
+    np.save(os.path.join(out_dir, "segment_target.npy"), np.array(rid, np.float64))
+    np.save(os.path.join(out_dir, "segment_index.npy"), np.array(idx, np.float64))
+    np.save(os.path.join(out_dir, "segment_length.npy"), np.array(lens, np.float64))
+    np.save(os.path.join(out_dir, "segment_bases.npy"), (np.concatenate(bases) if bases else np.zeros(0, np.uint8)).astype(np.float32))
 
 
 def main():
@@ -367,7 +399,7 @@ def main():
     harness.run(cut[n_steps - 1], cut[n_steps], 1, harness.windowing(cut[n_steps - 1], cut[n_steps], wthr))  # same entry as `e2e`
     st_full = ctx.stats()
     # ---- region 2: device stages only, inputs resident in HBM (one launch's working set is GBs of matrices + activations,
-    #      larger than the 126 MB L2, so no L2 flush is needed)
+    #      larger than the 50 MB L2 of an H100, so no L2 flush is needed)
     last_launch_bases = st_full["last_launch_bases"]
     barrier()
     ms_dev = ctx.replay_last_launch(args.steps)
@@ -376,6 +408,8 @@ def main():
     if rank == 0:
         sampler.join(timeout=3)
     st2 = ctx.stats()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ctx, harness, cut[n_steps - 1], cut[n_steps], args.dump_outputs)
     t_dev = ms_dev / 1e3
     vals = torch.tensor([t_dev, t_e2e, float(last_launch_bases * args.steps), float(r_e2e["bases"]), t_e2e_w, t_upload, t_gen,
                          float(st["host_allocs"]), float(st["windows"]), float(hi - lo)], dtype=torch.float64, device="cuda")
@@ -401,32 +435,21 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
-        tf_peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0))
-        peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+        # fallbacks: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s at up to 700 W)
+        hbm_peak = peaks.get("hbm_gbs", 3350.0)
+        tf_peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0))
+        peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet"
         mk, nk, cf = st_full["ms_kernel"], st_full["n_kernel"], st_full["class_flops"]
         # the dominant kernel of the step, by CUDA-event time of the isolated full-size launch
         KERNEL_OF = {"gemm": "k_gemm_ws", "ffn": "k_ffn_ws", "qkv_attn": "k_qkv_attn_ws", "stem": "k_stem_tc", "pileup": "k_pileup"}
-        DESCR = {"gemm": "tcgen05 bf16x3 contractions: out-proj(+LN) and read-axis collapse",
-                 "ffn": "fused FFN1 -> ReLU -> FFN2 + residual + LayerNorm on tcgen05, bf16x3",
-                 "qkv_attn": "fused QKV projection (tcgen05) + read-axis attention (mma.sync), bf16x3",
-                 "stem": "embedding+conv stem as a tcgen05 contraction (2 passes) + first LayerNorm",
+        DESCR = {"gemm": "wgmma bf16x3 contractions: out-proj(+LN) and read-axis collapse",
+                 "ffn": "fused FFN1 -> ReLU -> FFN2 + residual + LayerNorm on wgmma, bf16x3",
+                 "qkv_attn": "fused QKV projection (wgmma) + read-axis attention (mma.sync), bf16x3",
+                 "stem": "embedding+conv stem as a wgmma contraction (2 passes) + first LayerNorm",
                  "pileup": "pileup build (consume bitmaps, 4-row groups; second get_supported, majority vote)"}
         top = max((k for k in mk if k in KERNEL_OF), key=lambda k: mk[k])
         pile_gbs = st_full["pileup_algo_bytes"] / (mk["pileup"] * 1e-3) / 1e9 if mk["pileup"] > 0 else 0.0
-        traffic, traffic_src = {}, None
-        for name in ("r02_traffic.json", "r01d_traffic.json"):
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", name)))
-                traffic_src = name
-                break
-            except Exception:
-                pass
-        import re
-        traffic = {re.sub(r"^void |<.*", "", k): v for k, v in traffic.items()}   # "void k_ffn_ws<1>" -> "k_ffn_ws"
-        t_top = traffic[KERNEL_OF[top]].get("dram_bytes_per_launch") if isinstance(traffic.get(KERNEL_OF[top]), dict) else None
-        tnote = (f"from file profiles/{traffic_src} ({traffic.get('_note', 'ncu --set full capture of another run')}); not measured in this run"
-                 ) if t_top is not None else None
+        t_top, tnote = None, "not measured"
         if top == "pileup":
             roof = {"kernel": "k_pileup (" + DESCR[top] + ")", "bound": "hbm", "achieved": pile_gbs, "peak": hbm_peak,
                     "unit": "GB/s", "frac": pile_gbs / hbm_peak, "traffic": t_top, "traffic_note": tnote, "peak_source": peak_src,
@@ -448,7 +471,7 @@ def main():
                        "windows_per_step_rank0": st_full["windows"], "supported_positions_per_step_rank0": st_full["supported"],
                        "sharding": (f"read-id shard of one read set over {world} GPUs (shard.shard_targets: contiguous, balanced by windows), "
                                     f"read store replicated, no collective") if world > 1 else "single GPU",
-                       "l2": "inputs larger than L2 (per-launch working set >> 126 MB)",
+                       "l2": "inputs larger than L2 (per-launch working set >> 50 MB)",
                        "host_feature_threads": nthr, "numa_node": numa[0] if numa else None, "host_cpus_of_rank": my_cpus,
                        "host_worker_busy_ms_per_launch": st["ms_worker_busy"] / nl,
                        "host_worker_gpu_wait_ms_per_launch": st["ms_worker_gpu_wait"] / nl,

@@ -6,7 +6,7 @@ offline, so this ctypes layer is the harness that plays `lib.rs::error_correctio
 alignments grouped by target (`(tid, Vec<Alignment>)`, src/overlaps.rs:371-373), windows,
 corrected segments — and calls exactly the entry points the Rust `mod ffi` would bind.
 
-Everything compute-related happens inside libherro_b200.so (CUDA, sm_100a).  There is no CPU
+Everything compute-related happens inside libherro_b200.so (CUDA, sm_90a).  There is no CPU
 fallback: constructing a Context without a CUDA device raises.
 """
 from __future__ import annotations
@@ -111,7 +111,7 @@ EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
-    """-> dict(max_abs_err, max_abs_ref, ms_tc, ms_simt): tcgen05 bf16x3 contraction vs fp32 SIMT."""
+    """-> dict(max_abs_err, max_abs_ref, ms_tc, ms_simt): wgmma bf16x3 contraction vs fp32 SIMT."""
     L = load_library()
     v = [C.c_float() for _ in range(4)]
     rc = L.hb_selftest_gemm(device, M, N, K, act, res, lda_extra, *[C.byref(x) for x in v])

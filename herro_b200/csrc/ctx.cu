@@ -505,8 +505,8 @@ int load_weights(hb_ctx* ctx, const char* path) {
          get("bc", D, wt.bc) && get("wb", 5 * (size_t)D, wt.wb) && get("bb", 5, wt.bb) && get("wi", D, wt.wi) &&
          get("bi", 1, wt.bi);
     if (!ok) return ctx->err.rfind("cuda", 0) == 0 ? HB_ERR_CUDA : HB_ERR_MODEL;
-    // bf16 hi/lo split of the contraction weights for the tcgen05 path (gemm_tc.cu)
-    if (cudaDeviceGetAttribute(&wt.num_sms, cudaDevAttrMultiProcessorCount, ctx->device) != cudaSuccess) wt.num_sms = 148;
+    // bf16 hi/lo split of the contraction weights for the wgmma path (gemm_tc.cu)
+    if (cudaDeviceGetAttribute(&wt.num_sms, cudaDevAttrMultiProcessorCount, ctx->device) != cudaSuccess) wt.num_sms = 132;
     auto split = [&](const float* w, size_t n, SplitW& s) -> bool {
         void *hi = nullptr, *lo = nullptr;
         if (split_weights(w, n, &hi, &lo) != cudaSuccess) { ctx->err = "cuda: weight split failed"; return false; }
@@ -1228,7 +1228,7 @@ int stage_target(hb_ctx* ctx, const PreparedTarget& P, const hb_overlap* ovl, ui
     // so the targets in flight (and the latency to the first launch) do not grow with the thread count
     const uint32_t lt = ctx->opt.launch_targets, ns = std::max(1u, ctx->n_slots.load(std::memory_order_relaxed));
     // ... but never less than 256 targets per launch (unless launch_targets itself is smaller): ~1 300 windows is what it takes to
-    // fill 148 SMs with the one-CTA-per-window feature kernels and to amortise the ~25 launches of a batch
+    // fill the 132 SMs of an H100 with the one-CTA-per-window feature kernels and to amortise the ~25 launches of a batch
     uint32_t thr = std::min(lt, std::max(ctx->min_launch, lt / ns));
     // slow start: with several submitting threads, the first hand-overs after a flush are small and grow geometrically (48, 72, 108, ...
     // targets, counted over all threads), so that the GPU has work a few milliseconds after the first submit instead of after a
@@ -1330,7 +1330,7 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         if (cudaDeviceGetDefaultMemPool(&pool, cuda_device) == cudaSuccess)
             cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
     }
-    if (features_configure(ctx->opt.window_size) != cudaSuccess) { ctx->err = "kernel attribute setup failed (not an sm_100a device?)"; return bail(HB_ERR_CUDA); }
+    if (features_configure(ctx->opt.window_size) != cudaSuccess) { ctx->err = "kernel attribute setup failed (not an sm_90a device?)"; return bail(HB_ERR_CUDA); }
     int rc = load_weights(ctx, model_path);
     if (rc) return bail(rc);
     ctx->generation = g_ctx_generation.fetch_add(1);
@@ -1789,7 +1789,7 @@ int hb_selftest_gemm(int cuda_device, uint32_t M, uint32_t N, uint32_t K, int ac
     void *ahi = nullptr, *alo = nullptr, *ohi = nullptr, *olo = nullptr;
     if (split_weights(dA, hA.size(), &ahi, &alo) != cudaSuccess) return HB_ERR_CUDA;
     if (cudaMalloc(&ohi, hR.size() * 2) != cudaSuccess || cudaMalloc(&olo, hR.size() * 2) != cudaSuccess) return HB_ERR_CUDA;
-    int num_sms = 148;
+    int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, cuda_device);
     GemmArgs ga{};
     ga.Ahi = (const __nv_bfloat16*)ahi; ga.Alo = (const __nv_bfloat16*)alo; ga.lda = lda;

@@ -1,4 +1,4 @@
-// features.cu — sm_100a kernels for the pileup ("features") and consensus stages.
+// features.cu — sm_90a kernels for the pileup ("features") and consensus stages.
 //
 // Reference semantics: src/features.rs:44-722 (extract_features and helpers),
 // src/inference.rs:214-268 (token map, target indices), src/consensus.rs:86-227.

@@ -73,7 +73,7 @@ __global__ void k_stem(BatchView b, FwdWeights wt, uint32_t n0, uint32_t npos, f
 }
 
 // ---- LayerNorm over C (eps 1e-5), one warp per token row; output as split bf16 (hi + lo), the
-//      A-operand format of the tcgen05 contractions (gemm_tc.cu) --------------------------------
+//      A-operand format of the wgmma contractions (gemm_tc.cu) --------------------------------
 __device__ __forceinline__ uint32_t pack_bf2(__nv_bfloat16 a, __nv_bfloat16 b) {
     return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
@@ -429,8 +429,6 @@ int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, 
     const bool no_fuse = wt.no_fuse_ln != 0;  // debugging aid / A-B parity test
     const bool fuse_ln = (C == 128) && !no_fuse;
     const bool stem_ln = fuse_ln && wt.stem_kblocks;
-    // fully fused graph: only k_stem_tc and k_ffn_ws<true> touch the residual stream, both as row owners -> tile-blocked X
-    const bool x_blocked = stem_ln && oproj_in_ffn(wt);
     if (stem_ln && T > (size_t)npos * TOK_PER_POS) {  // rows of the pad positions: defined operands for the contractions
         const size_t off = (size_t)npos * TOK_PER_POS * C, n = (T - (size_t)npos * TOK_PER_POS) * C;
         cudaMemsetAsync(ws.Hhi + off, 0, n * sizeof(__nv_bfloat16), st);
@@ -441,7 +439,6 @@ int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, 
         StemArgs sa{(const __nv_bfloat16*)wt.s_stem.hi, (const __nv_bfloat16*)wt.s_stem.lo, (uint32_t)wt.stem_kblocks * 64,
                     (uint32_t)wt.stem_kblocks, (uint32_t)wt.stem_k, wt.stem_b, wt.read_pos, ws.X, n0, npos};
         if (stem_ln) { sa.ln_g = wt.layer[0].ln1_g; sa.ln_b = wt.layer[0].ln1_b; sa.out_hi = ws.Hhi; sa.out_lo = ws.Hlo; }
-        sa.x_blocked = x_blocked;
         stem_tc(b, sa, wt.num_sms, st);
     } else {
         k_stem<<<npos, (C + 31) / 32 * 32, stem_smem, st>>>(b, wt, n0, npos, ws.X);
@@ -490,7 +487,6 @@ int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, 
             if (oproj_in_ffn(wt)) {
                 fa.Wohi = (const __nv_bfloat16*)ly.s_o.hi; fa.Wolo = (const __nv_bfloat16*)ly.s_o.lo;
                 fa.bo = ly.bo; fa.ln2_g = ly.ln2_g; fa.ln2_b = ly.ln2_b;
-                fa.x_blocked = x_blocked;
             }
             kt.begin(K_FFN); ffn_tc(fa, wt.num_sms, st); kt.end(); nl++;
             continue;

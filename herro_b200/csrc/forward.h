@@ -70,11 +70,6 @@ struct FfnArgs {  // k_ffn_ws: fused FFN for C == 128, F == 512
     const __nv_bfloat16 *Wohi = nullptr, *Wolo = nullptr;  // [128][128]
     const float *bo = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
     int store_x = 1;  // 0: do not write the updated residual stream back (last layer: only LayerNorm(X) is consumed)
-    // 1: X is tile-blocked, [tile of 128 rows][32 chunks of 4 columns][128 rows][4 floats], so that the row-owner threads of the
-    // epilogues (one TMEM lane = one row each) read and write it with coalesced 16-byte accesses (a warp = 32 consecutive rows
-    // of one chunk = 512 contiguous bytes) and no shared-memory transposes.  Only in the fully fused graph, where k_stem_tc and
-    // k_ffn_ws<true> are the only kernels that touch X (forward.cu).
-    int x_blocked = 0;
 };
 cudaError_t ffn_tc(const FfnArgs& a, int num_sms, cudaStream_t st);
 struct QkvAttnArgs {  // k_qkv_attn_ws: QKV projection + read-axis attention for C == 128, 4 heads
@@ -94,7 +89,6 @@ struct StemArgs {  // k_stem_tc: the stem as a contraction over taps x 16 featur
     uint32_t n0, npos;               // work-list range
     const float *ln_g = nullptr, *ln_b = nullptr;          // optional: LayerNorm(X) of every row, emitted as split bf16
     __nv_bfloat16 *out_hi = nullptr, *out_lo = nullptr;    // [positions*32][128]; nullptr: X only
-    int x_blocked = 0;                                     // X in the tile-blocked layout (FfnArgs::x_blocked)
 };
 cudaError_t stem_tc(const BatchView& b, const StemArgs& a, int num_sms, cudaStream_t st);
 cudaError_t split_weights(const float* w, size_t n, void** hi, void** lo);

@@ -1,29 +1,25 @@
-// gemm_tc.cu — the dense contractions of the forward on the 5th-gen tensor cores (tcgen05).
+// gemm_tc.cu — the dense contractions of the forward on the Hopper tensor cores (wgmma).
 //
 //   D[M,N] = A[M,K] · W[N,K]^T  (+ bias, ReLU, residual, per the epilogue mode)      fp32 accumulate
 //
 // Precision: the north_star bound is 1e-3 absolute on fp32 logits, which a single bf16 pass
 // (2^-9 operand rounding over ~9 chained contractions) does not meet.  Every fp32 operand x is
-// carried as two bf16 terms x = hi + lo (lo = bf16(x - hi)); three tcgen05.mma passes accumulate
-// hi·hi + lo·hi + hi·lo in the fp32 TMEM accumulator (the dropped lo·lo term is 2^-18 relative).
+// carried as two bf16 terms x = hi + lo (lo = bf16(x - hi)); three wgmma passes accumulate
+// hi·hi + lo·hi + hi·lo in the fp32 register accumulator (the dropped lo·lo term is 2^-18 relative).
 // Weights are split once at load; activations are produced already split by the kernel that
 // writes them (LayerNorm, attention, the FFN1 epilogue), so operand staging is pure copying.
 //
 // Kernels (all persistent, warp-specialised, one CTA per SM; operands as K-major SWIZZLE_128B shared-memory tiles):
 //   k_gemm_ws      D = A·W^T with bias / ReLU / residual / LayerNorm epilogues (out-proj, read-axis collapse, fallbacks)
 //   k_ffn_ws       FFN1 -> ReLU -> FFN2 + residual + LayerNorm, hidden activations kept on chip
-//   k_qkv_attn_ws  QKV projection (tcgen05) + per-position attention (mma.sync) in the epilogue warps
+//   k_qkv_attn_ws  QKV projection (wgmma) + per-position attention (mma.sync)
 //   k_stem_tc      embedding + conv stem as a contraction, A tile synthesised from the pileup matrix, + first LayerNorm
-// Common skeleton (k_gemm_ws, 320 threads):
-//   warps 0-7  two epilogue warpgroups: warp & 3 = TMEM lane quadrant (one position = 32 read tokens), warp >> 2 = column
-//              half; tcgen05.ld, bias / ReLU / residual / LayerNorm / bf16 split; global accesses transposed through
-//              per-warp shared-memory buffers so every instruction covers whole row segments
-//   warp  8    one lane issues TMA (cp.async.bulk.tensor.2d) for the A and W k-block tiles into a 3-stage ring
-//   warp  9    one lane issues tcgen05.mma (M=128, N=128, K=16; 12 per k-block), tcgen05.commit releases ring stages and
-//              publishes the accumulator
-// Two TMEM accumulators (2 x 128 columns) let the epilogue of item i overlap the MMAs of i+1.
-// Work items (m_tile, n_chunk) are dealt round-robin so CTAs working on the same m_tile share
-// its A tile in L2.
+// Common skeleton: two consumer warpgroups (warps 0-7) and one producer warp (warp 8, one lane issues TMA into a ring of
+// k-block stages guarded by full / empty mbarriers).  A work item is a tile of 128 rows; consumer warpgroup wg issues
+// wgmma.m64nNk16 for rows [64 wg, 64 wg + 64) and runs the epilogue on its own accumulator fragments:
+// thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 and that + 8, columns 8 j + 2 (t % 4) + {0, 1}
+// (acc[4 j], acc[4 j + 1] for the first row, acc[4 j + 2], acc[4 j + 3] for the second).  A row's 128 columns live in
+// the 4 lanes of a quad, so a LayerNorm reduces with two shuffles.
 #include <cstdio>
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -37,10 +33,7 @@ namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64, STAGES = 3;
 constexpr int STAGE_BYTES = (2 * BM + 2 * BN) * 128;  // A hi/lo + W hi/lo tiles of one k-block: 64 KB
-// k_gemm_ws / k_ffn_ws: the epilogue is the critical path (4 warps could not keep up with the tensor pipe), so two
-// epilogue warpgroups split the 128 columns of an accumulator: warps 0-7 epilogue (warp & 3 = TMEM lane quadrant,
-// warp >> 2 = column half), warp 8 TMA producer, warp 9 MMA
-constexpr int G_EPI = 256, G_THREADS = 320, G_PROD_WARP = 8, G_MMA_WARP = 9;  // operands arrive by TMA: one producer lane
+constexpr int C_THREADS = 256, G_THREADS = 288, G_PROD_WARP = 8;  // consumers: warps 0-7 (two warpgroups); producer: warp 8
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -62,64 +55,83 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "}" ::"r"(smem_u32(bar)), "r"(parity)
         : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    // arrives once all tcgen05.mma issued so far by this thread have completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// TMA: one thread copies a [128 rows x 64 bf16] box of a 2-D tensor into a SWIZZLE_128B shared-memory tile
-// (the layout the UMMA descriptors expect) and completes `bytes` on the mbarrier
+// TMA: one thread copies a [rows x 64 bf16] box of a 2-D tensor into a SWIZZLE_128B shared-memory tile
+// (the layout the wgmma descriptors expect) and completes `bytes` on the mbarrier
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint64_t* bar, int c_inner, int c_row) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
                  "l"((uint64_t)tm), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_row)
                  : "memory");
 }
-// TMA store of one SWIZZLE_128B [128 rows x 64 bf16] shared-memory tile into a 2-D tensor (bulk async-group completion)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t src, int c_inner, int c_row) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"((uint64_t)tm), "r"(src), "r"(c_inner),
-                 "r"(c_row)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }  // sources may be overwritten
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// pull a line towards L2 ahead of the (latency-exposed) row-owner loads of an epilogue
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
+// named barrier over `n` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// generic-proxy shared-memory writes -> visible to the tensor core (async proxy)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout)
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma layout): start address, LBO (unused for a swizzled
+// K-major operand that is one atom wide along K), SBO = 8 rows * 128 B, layout type 1 = SWIZZLE_128B.  Tiles are
+// 1024-byte aligned, so the base offset is 0; a step of 16 along K inside the atom adds 32 bytes to the start address.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3ffffu) >> 4);  // start address, 16-byte units, bits [0,14)
-    d |= (uint64_t)(1024u >> 4) << 32;         // SBO = 8 rows * 128 B, bits [32,46); LBO unused (one atom along K)
-    d |= (uint64_t)1 << 46;                    // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                    // layout type SWIZZLE_128B
+    d |= (uint64_t)((saddr & 0x3ffffu) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024u >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 
-// instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, M=128, N=128
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&a)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(a[i])::"memory");
+}
 
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] · B[128 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulator in registers
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+// D[64 x 96] (+)= A[64 x 16] · B[96 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulator in registers
+__device__ __forceinline__ void wgmma_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+        "%48, %49, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
 
-__device__ __forceinline__ uint32_t pack2(__nv_bfloat16 a, __nv_bfloat16 b) {
-    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+// one 64-wide k-block of split operands: hi·hi + lo·hi + hi·lo (4 k-steps of 16), committed as one wgmma group
+__device__ __forceinline__ void mma_kblock(float (&acc)[64], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, bool zero) {
+    const uint64_t dAh = make_desc(a_hi), dAl = make_desc(a_lo), dBh = make_desc(b_hi), dBl = make_desc(b_lo);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; k++) {
+        const uint64_t adv = (uint64_t)(k * 2);  // +32 bytes along K inside the swizzle atom
+        wgmma_n128(acc, dAh + adv, dBh + adv, (zero && k == 0) ? 0u : 1u);
+        wgmma_n128(acc, dAl + adv, dBh + adv, 1u);
+        wgmma_n128(acc, dAh + adv, dBl + adv, 1u);
+    }
+    wg_commit();
 }
-// split two floats into packed bf16x2 hi and lo words with the 2-wide convert (F2FP.PACK_AB, full-rate ALU) instead of
-// four scalar F2F conversions: hi = bf16(x), lo = bf16(x - hi)
+
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    // hi = bf16(x), lo = bf16(x - hi), two values per 2-wide convert
     const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
     hi = *reinterpret_cast<const uint32_t*>(&h);
     const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
@@ -127,95 +139,82 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 fp32 columns of this thread's TMEM lane (its row) written back: parks a row of the residual stream on chip
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),
-        "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]),
-        "r"(v[31])
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// ---- row-owner <-> coalesced transposes through a per-warp shared-memory buffer ---------------------------------------
-// In the epilogues a thread owns one row (its TMEM lane).  Touching global memory directly from that layout issues
-// warp instructions that hit 32 different rows with 16 bytes each (32 partial sectors): measured 2x slower kernels.
-// These helpers move 16 fp32 (or 16 bf16) columns of the warp's 32 rows through a swizzled [32][64 B] buffer so that
-// every global instruction covers whole 64-byte (fp32) / 32-byte (bf16) row segments.
-__device__ __forceinline__ void warp_store_f32x16(float* stg, int lane, float* gbase, size_t ld, const float* v) {
+// ---- epilogue helpers on a [64 x 128] accumulator fragment (see the layout above) ------------------------------------
+// LayerNorm statistics (eps 1e-5) of the thread's two rows: mean and 1/std, the row sums completed across the lane quad
+__device__ __forceinline__ void frag_ln_stats(const float (&a)[64], float& m0, float& r0, float& m1, float& r1) {
+    float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-    for (int cq = 0; cq < 4; cq++)
-        *(float4*)(stg + lane * 16 + ((cq ^ ((lane >> 1) & 3)) << 2)) = make_float4(v[cq * 4], v[cq * 4 + 1], v[cq * 4 + 2], v[cq * 4 + 3]);
-    __syncwarp();
+    for (int j = 0; j < 16; j++) { s0 += a[4 * j] + a[4 * j + 1]; s1 += a[4 * j + 2] + a[4 * j + 3]; }
+    s0 += __shfl_xor_sync(HB_FULL, s0, 1); s0 += __shfl_xor_sync(HB_FULL, s0, 2);
+    s1 += __shfl_xor_sync(HB_FULL, s1, 1); s1 += __shfl_xor_sync(HB_FULL, s1, 2);
+    m0 = s0 * (1.f / BN); m1 = s1 * (1.f / BN);
+    float v0 = 0.f, v1 = 0.f;
 #pragma unroll
-    for (int jj = 0; jj < 4; jj++) {
-        const int rr = jj * 8 + (lane >> 2), cq = lane & 3;
-        *(float4*)(gbase + (size_t)rr * ld + cq * 4) = *(const float4*)(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2));
+    for (int j = 0; j < 16; j++) {
+        float d = a[4 * j] - m0; v0 = fmaf(d, d, v0);
+        d = a[4 * j + 1] - m0; v0 = fmaf(d, d, v0);
+        d = a[4 * j + 2] - m1; v1 = fmaf(d, d, v1);
+        d = a[4 * j + 3] - m1; v1 = fmaf(d, d, v1);
     }
-    __syncwarp();
+    v0 += __shfl_xor_sync(HB_FULL, v0, 1); v0 += __shfl_xor_sync(HB_FULL, v0, 2);
+    v1 += __shfl_xor_sync(HB_FULL, v1, 1); v1 += __shfl_xor_sync(HB_FULL, v1, 2);
+    r0 = rsqrtf(v0 * (1.f / BN) + 1e-5f); r1 = rsqrtf(v1 * (1.f / BN) + 1e-5f);
 }
-// the two halves of warp_load_f32x16, so that the global loads of the next block can be in flight while the current one is
-// consumed: warp_ldg_f32x16 issues the 4 coalesced 16-byte loads, warp_xpose_f32x16 turns them into the lane's own row
-__device__ __forceinline__ void warp_ldg_f32x16(int lane, const float* gbase, size_t ld, float4 (&t)[4]) {
+// LayerNorm of the thread's two rows, in place
+__device__ __forceinline__ void frag_layernorm(float (&a)[64], const float* gam, const float* bet, int fc) {
+    float m0, r0, m1, r1;
+    frag_ln_stats(a, m0, r0, m1, r1);
 #pragma unroll
-    for (int jj = 0; jj < 4; jj++) t[jj] = *(const float4*)(gbase + (size_t)(jj * 8 + (lane >> 2)) * ld + (lane & 3) * 4);
+    for (int j = 0; j < 16; j++) {
+        const int c = 8 * j + fc;
+        const float g0 = gam[c], g1 = gam[c + 1], b0 = bet[c], b1 = bet[c + 1];
+        a[4 * j] = (a[4 * j] - m0) * r0 * g0 + b0;
+        a[4 * j + 1] = (a[4 * j + 1] - m0) * r0 * g1 + b1;
+        a[4 * j + 2] = (a[4 * j + 2] - m1) * r1 * g0 + b0;
+        a[4 * j + 3] = (a[4 * j + 3] - m1) * r1 * g1 + b1;
+    }
 }
-__device__ __forceinline__ void warp_xpose_f32x16(float* stg, int lane, const float4 (&t)[4], float* v) {
+// fp32 rows -> row-major global [.., ld] at column c0 (a quad writes 32 contiguous bytes of a row)
+__device__ __forceinline__ void frag_store_f32(const float (&a)[64], float* base, size_t ld, size_t row0, int c0, int fc) {
 #pragma unroll
-    for (int jj = 0; jj < 4; jj++) {
-        const int rr = jj * 8 + (lane >> 2), cq = lane & 3;
-        *(float4*)(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2)) = t[jj];
+    for (int j = 0; j < 16; j++) {
+        *(float2*)(base + row0 * ld + c0 + 8 * j + fc) = make_float2(a[4 * j], a[4 * j + 1]);
+        *(float2*)(base + (row0 + 8) * ld + c0 + 8 * j + fc) = make_float2(a[4 * j + 2], a[4 * j + 3]);
     }
-    __syncwarp();
-#pragma unroll
-    for (int cq = 0; cq < 4; cq++) {
-        const float4 u = *(const float4*)(stg + lane * 16 + ((cq ^ ((lane >> 1) & 3)) << 2));
-        v[cq * 4] = u.x; v[cq * 4 + 1] = u.y; v[cq * 4 + 2] = u.z; v[cq * 4 + 3] = u.w;
-    }
-    __syncwarp();
 }
-__device__ __forceinline__ void warp_load_f32x16(float* stg, int lane, const float* gbase, size_t ld, float* v) {
+// fp32 rows -> split bf16 row-major global arrays
+__device__ __forceinline__ void frag_store_split(const float (&a)[64], __nv_bfloat16* hi, __nv_bfloat16* lo, size_t ld, size_t row0, int c0,
+                                                 int fc) {
 #pragma unroll
-    for (int jj = 0; jj < 4; jj++) {
-        const int rr = jj * 8 + (lane >> 2), cq = lane & 3;
-        *(float4*)(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2)) = *(const float4*)(gbase + (size_t)rr * ld + cq * 4);
+    for (int j = 0; j < 16; j++) {
+        uint32_t h, l;
+        const size_t o0 = row0 * ld + c0 + 8 * j + fc, o1 = (row0 + 8) * ld + c0 + 8 * j + fc;
+        split2(a[4 * j], a[4 * j + 1], h, l);
+        *(uint32_t*)(hi + o0) = h; *(uint32_t*)(lo + o0) = l;
+        split2(a[4 * j + 2], a[4 * j + 3], h, l);
+        *(uint32_t*)(hi + o1) = h; *(uint32_t*)(lo + o1) = l;
     }
-    __syncwarp();
-#pragma unroll
-    for (int cq = 0; cq < 4; cq++) {
-        const float4 t = *(const float4*)(stg + lane * 16 + ((cq ^ ((lane >> 1) & 3)) << 2));
-        v[cq * 4] = t.x; v[cq * 4 + 1] = t.y; v[cq * 4 + 2] = t.z; v[cq * 4 + 3] = t.w;
-    }
-    __syncwarp();
 }
-// 16 bf16 columns (8 packed words per row) of the warp's 32 rows; buffer viewed as [32 rows][8 words]
-__device__ __forceinline__ void warp_store_bf16x16(uint32_t* stg, int lane, __nv_bfloat16* gbase, size_t ld, const uint32_t* w) {
-    *(uint4*)(stg + lane * 8 + (((lane >> 2) & 1) << 2)) = make_uint4(w[0], w[1], w[2], w[3]);
-    *(uint4*)(stg + lane * 8 + ((((lane >> 2) & 1) ^ 1) << 2)) = make_uint4(w[4], w[5], w[6], w[7]);
-    __syncwarp();
+// fp32 rows -> split bf16 into an operand tile in shared memory ([kb][hi|lo][128 rows x 128 B], SWIZZLE_128B), row r = tile row.
+// With `gam`, the rows are written LayerNorm-ed with the statistics ln = {mean0, rstd0, mean1, rstd1} (a is left as it is).
+__device__ __forceinline__ void frag_store_tile(const float (&a)[64], uint8_t* tile, int r, int fc, const float* gam = nullptr,
+                                                const float* bet = nullptr, const float* ln = nullptr) {
 #pragma unroll
-    for (int jj = 0; jj < 2; jj++) {
-        const int rr = jj * 16 + (lane >> 1), cq = lane & 1;
-        *(uint4*)(gbase + (size_t)rr * ld + cq * 8) = *(const uint4*)(stg + rr * 8 + ((cq ^ ((rr >> 2) & 1)) << 2));
-    }
-    __syncwarp();
+    for (int j = 0; j < 16; j++)
+#pragma unroll
+        for (int hf = 0; hf < 2; hf++) {
+            const int rr = r + 8 * hf, c = 8 * j + fc;
+            float x = a[4 * j + 2 * hf], y = a[4 * j + 2 * hf + 1];
+            if (gam) {
+                x = (x - ln[2 * hf]) * ln[2 * hf + 1] * gam[c] + bet[c];
+                y = (y - ln[2 * hf]) * ln[2 * hf + 1] * gam[c + 1] + bet[c + 1];
+            }
+            uint32_t h, l;
+            split2(x, y, h, l);
+            const uint32_t off = (uint32_t)(j >> 3) * (2 * BM * 128) + (uint32_t)rr * 128u + (uint32_t)((((j & 7) ^ (rr & 7)) << 4) + fc * 2);
+            *(uint32_t*)(tile + off) = h;
+            *(uint32_t*)(tile + off + BM * 128) = l;
+        }
 }
 
 }  // namespace
@@ -226,30 +225,16 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_ws(GemmArgs g, const __gr
     extern __shared__ uint8_t smem_dyn[];
     // SWIZZLE_128B operands need 1024-byte alignment; the dynamic segment starts after the static one
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], tfull_bar[2], tempty_bar[2];
-    __shared__ uint32_t tmem_base_s;
-    // per-item bias chunk and the LayerNorm affine: read from shared memory in the epilogue (the L1 of this
-    // kernel is almost entirely carved out for the operand ring, so repeated global reads would pay L2 latency)
-    __shared__ __align__(16) float s_bias[2][BN], s_lng[BN], s_lnb[BN];
-    __shared__ float s_red[2][2][BM];  // [item parity][column half][row]: LayerNorm partial sums
-    // per-warp transpose buffers [32 rows][16 floats]: a thread owns a row of the accumulator, but global stores are issued
-    // with lanes covering whole 64-byte row segments (sector-complete, 8 rows per instruction) instead of 32 scattered 16-byte pieces
-    __shared__ __align__(16) float s_stage[8][32 * 16];
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
+    __shared__ __align__(16) float s_lng[BN], s_lnb[BN];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(2 * BN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], G_EPI); }
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C_THREADS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (g.mode == GEMM_OUT_F32_RES_LN && tid < BN) { s_lng[tid] = g.ln_g[tid]; s_lnb[tid] = g.ln_b[tid]; }
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
 
     const uint32_t n_items = g.m_tiles * g.n_chunks;
     const uint32_t kbs = g.k_blocks;
@@ -273,702 +258,233 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_ws(GemmArgs g, const __gr
                 }
             }
         }
-    } else if (warp == G_MMA_WARP) {
-        // =============================== MMA issuer ===============================
-        if (lane == 0) {
-            uint32_t it_stage = 0, n_done = 0;
-            for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
-                const uint32_t acc = n_done & 1, aph = (n_done >> 1) & 1;
-                mbar_wait(&tempty_bar[acc], aph ^ 1);  // epilogue has drained this accumulator
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (uint32_t kb = 0; kb < kbs; kb++, it_stage++) {
-                    const uint32_t s = it_stage % STAGES, ph = (it_stage / STAGES) & 1;
-                    mbar_wait(&full_bar[s], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t sb = smem_u32(smem + (size_t)s * STAGE_BYTES);
-                    const uint64_t dAh = make_desc(sb), dAl = make_desc(sb + BM * 128);
-                    const uint64_t dBh = make_desc(sb + 2 * BM * 128), dBl = make_desc(sb + 2 * BM * 128 + BN * 128);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; k++) {
-                        const uint64_t adv = (uint64_t)((k * 32) >> 4);  // +32 bytes along K inside the swizzle atom
-                        mma_bf16(tmem_d, dAh + adv, dBh + adv, (kb | (uint32_t)k) ? 1u : 0u);
-                        mma_bf16(tmem_d, dAl + adv, dBh + adv, 1u);
-                        mma_bf16(tmem_d, dAh + adv, dBl + adv, 1u);
-                    }
-                    umma_commit(&empty_bar[s]);  // ring stage reusable once these MMAs have read it
-                }
-                umma_commit(&tfull_bar[acc]);    // accumulator complete
-            }
-        }
-    } else {
-        // =============================== epilogue: 8 warps, 64 columns each =======================
-        const int wq = warp & 3, eh = warp >> 2;  // TMEM lane quadrant, column half
-        const int ch = eh * 64;                   // first of this thread's 64 columns inside the 128-wide item
-        if (g.mode == GEMM_OUT_F32_RES_LN && tid < BN) { s_lng[tid] = g.ln_g[tid]; s_lnb[tid] = g.ln_b[tid]; }
-        if ((g.mode == GEMM_OUT_F32_RES_LN || g.mode == GEMM_OUT_F32_RES) && blockIdx.x < n_items) {
-            const uint32_t fm0 = (blockIdx.x / g.n_chunks) * BM, fn0 = (blockIdx.x % g.n_chunks) * BN;
-            const float* pr = g.res + ((size_t)fm0 + wq * 32 + lane) * g.ldc + fn0 + ch;
-            prefetch_l2(pr); prefetch_l2(pr + 32);
-        }
-        uint32_t n_done = 0;
-        for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
-            const uint32_t m0 = (item / g.n_chunks) * BM, n0 = (item % g.n_chunks) * BN;
-            const uint32_t acc = n_done & 1, aph = (n_done >> 1) & 1;
-            if ((g.mode == GEMM_OUT_F32_RES_LN || g.mode == GEMM_OUT_F32_RES) && item + gridDim.x < n_items) {
-                // the residual rows of the next item: in L2 by the time its epilogue loads them (thread = row, 64 columns = 2 lines)
-                const uint32_t nm0 = ((item + gridDim.x) / g.n_chunks) * BM, nn0 = ((item + gridDim.x) % g.n_chunks) * BN;
-                const float* pr = g.res + ((size_t)nm0 + (warp & 3) * 32 + lane) * g.ldc + nn0 + (warp >> 2) * 64;
-                prefetch_l2(pr); prefetch_l2(pr + 32);
-            }
-            if (tid < BN) s_bias[acc][tid] = g.bias[n0 + tid];  // the previous user of this slot finished 2 items ago
-            asm volatile("bar.sync 2, 256;" ::: "memory");       // epilogue warps only
-            const float* sb = s_bias[acc] + ch;
-            float4 pre[4];  // residual block in flight (software pipelined: the next block loads while this one is consumed)
-            if (g.mode == GEMM_OUT_F32_RES_LN)  // the first one is requested before the wait for the MMAs: it does not depend on them
-                warp_ldg_f32x16(lane, g.out + ((size_t)m0 + wq * 32) * g.ldc + ch, g.ldc, pre);
-            mbar_wait(&tfull_bar[acc], aph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t r = wq * 32 + lane;
-            const size_t row = (size_t)m0 + r;
-            const uint32_t taddr = tmem_base + acc * BN + ch + ((uint32_t)(wq * 32) << 16);
-            if (g.mode == GEMM_OUT_F32_RES_LN) {
-                // residual add + fp32 store of this thread's half row, then LayerNorm of the whole row with the
-                // partial sums exchanged with the thread that owns the other half
-                float x[64];
-                float* stg = s_stage[warp];
-                float* xblk = g.out + ((size_t)m0 + wq * 32) * g.ldc + ch;  // this warp's [32 rows][64 cols] block of X
-#pragma unroll
-                for (int c0 = 0; c0 < 64; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(taddr + (uint32_t)c0, v);
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        float rv[16];
-                        warp_xpose_f32x16(stg, lane, pre, rv);
-                        if (c0 + h * 16 + 16 < 64) warp_ldg_f32x16(lane, xblk + c0 + h * 16 + 16, g.ldc, pre);
-#pragma unroll
-                        for (int j = 0; j < 16; j++) x[c0 + h * 16 + j] = __uint_as_float(v[h * 16 + j]) + sb[c0 + h * 16 + j] + rv[j];
-                        warp_store_f32x16(stg, lane, xblk + c0 + h * 16, g.ldc, x + c0 + h * 16);
-                    }
-                }
-                // TMEM is drained: let the MMA warp start the next item while this thread normalises
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(&tempty_bar[acc]);
-                float sum = 0.f;
-#pragma unroll
-                for (int j = 0; j < 64; j++) sum += x[j];
-                s_red[acc][eh][r] = sum;
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float mean = (s_red[acc][0][r] + s_red[acc][1][r]) * (1.f / BN);
-                float var = 0.f;
-#pragma unroll
-                for (int j = 0; j < 64; j++) { const float d = x[j] - mean; var = fmaf(d, d, var); }
-                asm volatile("bar.sync 2, 256;" ::: "memory");  // both halves have read the sums
-                s_red[acc][eh][r] = var;
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float rstd = rsqrtf((s_red[acc][0][r] + s_red[acc][1][r]) * (1.f / BN) + 1e-5f);
-                __nv_bfloat16* hblk = g.out_hi + ((size_t)m0 + wq * 32) * g.ldo + ch;
-                __nv_bfloat16* lblk = g.out_lo + ((size_t)m0 + wq * 32) * g.ldo + ch;
-#pragma unroll
-                for (int j = 0; j < 64; j += 16) {
-                    uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        const float a = (x[j + e] - mean) * rstd * s_lng[ch + j + e] + s_lnb[ch + j + e];
-                        const float b = (x[j + e + 1] - mean) * rstd * s_lng[ch + j + e + 1] + s_lnb[ch + j + e + 1];
-                        split2(a, b, hi[e >> 1], lo[e >> 1]);
-                    }
-                    warp_store_bf16x16((uint32_t*)stg, lane, hblk + j, g.ldo, hi);
-                    warp_store_bf16x16((uint32_t*)stg, lane, lblk + j, g.ldo, lo);
-                }
-                continue;
-            }
-#pragma unroll 1
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(taddr + (uint32_t)c0, v);
-                const int col = (int)n0 + ch + c0;
-                float o[32];
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 bv = *(const float4*)(sb + c0 + j);
-                    o[j] = __uint_as_float(v[j]) + bv.x; o[j + 1] = __uint_as_float(v[j + 1]) + bv.y;
-                    o[j + 2] = __uint_as_float(v[j + 2]) + bv.z; o[j + 3] = __uint_as_float(v[j + 3]) + bv.w;
-                }
-                if (g.mode == GEMM_OUT_SPLIT_RELU) {
-                    uint32_t hi[16], lo[16];
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) split2(fmaxf(o[j], 0.f), fmaxf(o[j + 1], 0.f), hi[j >> 1], lo[j >> 1]);
-                    uint4* ph = (uint4*)(g.out_hi + row * g.ldo + col);
-                    uint4* pl = (uint4*)(g.out_lo + row * g.ldo + col);
-#pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        ph[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-                        pl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
-                    }
-                } else {
-                    float* stg = s_stage[warp];
-                    float* gbase = g.out + ((size_t)m0 + wq * 32) * g.ldc + col;  // row 0 of this warp's 32-row block
-                    if (g.mode == GEMM_OUT_F32_RES) {
-                        const float* rbase = g.res + ((size_t)m0 + wq * 32) * g.ldc + col;
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            float rv[16];
-                            warp_load_f32x16(stg, lane, rbase + h * 16, g.ldc, rv);
-#pragma unroll
-                            for (int j = 0; j < 16; j++) o[h * 16 + j] += rv[j];
-                        }
-                    } else if (g.mode == GEMM_OUT_F32_RELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) o[j] = fmaxf(o[j], 0.f);
-                    }
-                    warp_store_f32x16(stg, lane, gbase, g.ldc, o);
-                    warp_store_f32x16(stg, lane, gbase + 16, g.ldc, o + 16);
-                }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&tempty_bar[acc]);
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * BN));
+    // =============================== consumers: wgmma over this warpgroup's 64 rows, then the epilogue ===============
+    const int wg = warp >> 2;
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), fc = (lane & 3) * 2;  // fragment row (tile-local) / column offset
+    uint32_t it_stage = 0;
+    float acc[64];
+    for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const uint32_t m0 = (item / g.n_chunks) * BM, n0 = (item % g.n_chunks) * BN;
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < kbs; kb++, it_stage++) {
+            const uint32_t s = it_stage % STAGES, ph = (it_stage / STAGES) & 1;
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sb = smem_u32(smem + (size_t)s * STAGE_BYTES);
+            mma_kblock(acc, sb + wg * 64 * 128, sb + BM * 128 + wg * 64 * 128, sb + 2 * BM * 128, sb + 2 * BM * 128 + BN * 128, kb == 0);
+            if (kb > 0) {  // the previous k-block's group has completed: its stage may be refilled
+                wg_wait<1>();
+                mbar_arrive(&empty_bar[prev]);
+            }
+            prev = s;
+        }
+        wg_wait<0>();
+        acc_fence(acc);
+        mbar_arrive(&empty_bar[prev]);
+        const size_t row0 = (size_t)m0 + fr;
+        if (g.mode == GEMM_OUT_F32_RES_LN) {
+            // residual add + fp32 store, then LayerNorm of the row -> split bf16 (N == 128: the whole row is in the quad)
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int c = 8 * j + fc;
+                const float2 bv = *(const float2*)(g.bias + c);
+                const float2 x0 = *(const float2*)(g.res + row0 * g.ldc + c), x1 = *(const float2*)(g.res + (row0 + 8) * g.ldc + c);
+                acc[4 * j] = acc[4 * j] + bv.x + x0.x; acc[4 * j + 1] = acc[4 * j + 1] + bv.y + x0.y;
+                acc[4 * j + 2] = acc[4 * j + 2] + bv.x + x1.x; acc[4 * j + 3] = acc[4 * j + 3] + bv.y + x1.y;
+            }
+            frag_store_f32(acc, g.out, g.ldc, row0, 0, fc);
+            frag_layernorm(acc, s_lng, s_lnb, fc);
+            frag_store_split(acc, g.out_hi, g.out_lo, g.ldo, row0, 0, fc);
+            continue;
+        }
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const int c = (int)n0 + 8 * j + fc;
+            const float2 bv = *(const float2*)(g.bias + c);
+            acc[4 * j] += bv.x; acc[4 * j + 1] += bv.y; acc[4 * j + 2] += bv.x; acc[4 * j + 3] += bv.y;
+            if (g.mode == GEMM_OUT_F32_RES) {
+                const float2 x0 = *(const float2*)(g.res + row0 * g.ldc + c), x1 = *(const float2*)(g.res + (row0 + 8) * g.ldc + c);
+                acc[4 * j] += x0.x; acc[4 * j + 1] += x0.y; acc[4 * j + 2] += x1.x; acc[4 * j + 3] += x1.y;
+            } else if (g.mode == GEMM_OUT_F32_RELU || g.mode == GEMM_OUT_SPLIT_RELU) {
+#pragma unroll
+                for (int e = 0; e < 4; e++) acc[4 * j + e] = fmaxf(acc[4 * j + e], 0.f);
+            }
+        }
+        if (g.mode == GEMM_OUT_SPLIT_RELU) frag_store_split(acc, g.out_hi, g.out_lo, g.ldo, row0, (int)n0, fc);
+        else frag_store_f32(acc, g.out, g.ldc, row0, (int)n0, fc);
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Fused FFN for C == 128:   X += W2 · relu(W1 · H + b1) + b2 ;  H' = LayerNorm(X) (split bf16)
-// The hidden activations never leave the SM: per 128-token tile and per 128-wide hidden chunk c,
-//   F1(c): accF[c&1] = H · W1[c]^T           (tcgen05, H tile resident in shared memory)
-//   E1(c): relu(accF + b1[c]) -> split bf16 -> swizzled K-major tile A2 in shared memory
+// The hidden activations never leave the SM: per 128-token tile and per 128-wide hidden chunk c, each consumer warpgroup
+// (64 rows) runs
+//   F1(c): accF = H · W1[c]^T           (H tile resident in shared memory)
+//   E1(c): relu(accF + b1[c]) -> split bf16 -> the warpgroup's rows of the swizzled K-major tile A2 in shared memory
 //   F2(c): accO += A2 · W2[:, c]^T
-// and one final epilogue (residual, fp32 store, LayerNorm, split-bf16 store).  W1/W2 k-block tiles stream
-// through the cp.async ring in issue order F1(0) F1(1) F2(0) F1(2) F2(1) F1(3) F2(2) F2(3), so E1(c)
-// overlaps the MMAs of F1(c+1).  Saves writing and re-reading the [T, F] hidden tensor (4 KB per token and layer).
+// accO starts as X + b2, so after F2(3) it holds the new residual row: one final epilogue stores it and its LayerNorm.
+// W k-block tiles stream through the TMA ring in issue order F1(0) F2(0) F1(1) F2(1) ... F2(3).  Saves writing and
+// re-reading the [T, F] hidden tensor (4 KB per token and layer).
+// FUSE_O: the attention out-projection, its residual add and LayerNorm (ln2) run in front of the FFN inside this kernel:
+//   P0   : accO = O · Wo^T                       (O = attention output tile, loaded where H used to be)
+//   E0   : accO = accO + bo + X (= X'), H = LN2(X') -> split bf16 -> written over the warpgroup's rows of the O tile
+//          (the A operand of FFN1); accO += b2 and the FFN accumulates on top of it.
+// This removes the HBM-bound out-projection kernel (it re-read and re-wrote the fp32 residual stream).
 // ------------------------------------------------------------------------------------------------
 constexpr int FFN_RING_BYTES = 2 * BN * 128;        // one W k-block tile, hi + lo: 32 KB
 constexpr int FFN_A_BYTES = 2 * 2 * BM * 128;       // a [128 x 128] operand as 2 k-blocks x (hi, lo): 64 KB
+constexpr int FFN_STAGES = 2;                       // 2 x 64 KB operand tiles + 2 x 32 KB ring = 192 KB
 
-// issue order of the 8 contractions of a tile: (is_F2, chunk)
-__device__ __forceinline__ void ffn_step(int i, int& is2, int& c) {
-    // 0:F1(0) 1:F1(1) 2:F2(0) 3:F1(2) 4:F2(1) 5:F1(3) 6:F2(2) 7:F2(3)
-    is2 = (0xD4 >> i) & 1;
-    c = (0xED84 >> (2 * i)) & 3;
-}
-constexpr int FFN_STAGES = 2;  // 2 x 64 KB operand tiles + 2 x 32 KB ring = 192 KB
-
-// FUSE_O: the attention out-projection, its residual add and LayerNorm (ln2) run in front of the FFN inside this kernel:
-//   P0   : accO = O · Wo^T                       (O = attention output tile, loaded where H used to be)
-//   E0   : X' = accO + bo + X  ->  parked in 128 spare TMEM columns (fp32, one row per lane);  H = LN2(X') -> split bf16 ->
-//          written over the O tile in shared memory (it is the A operand of FFN1)
-//   ...  : FFN as above, and the final epilogue takes its residual X' from TMEM instead of HBM.
-// This removes the HBM-bound out-projection kernel (it re-read and re-wrote the fp32 residual stream: 256 KB per 128-token
-// tile and layer).  Cost: accO is single-buffered (its second buffer holds X'), so the next tile's P0 waits for this tile's
-// final epilogue to drain the accumulator.
-// Per-role timeline of two tiles of block 0 (clock64), compiled in with -DHB_FFN_TRACE and printed by ffn_tc on its 25th call:
-// how the numbers in DESIGN.md 4.3 (who waits for whom inside a tile) were obtained.  Not part of the product build.
-#ifdef HB_FFN_TRACE
-__device__ unsigned long long hb_ffn_trace[3][2][64];  // [role: 0 MMA, 1 epilogue thread 0, 2 producer][tile 10/11][event]
-#define TR(role, k) do { if (blockIdx.x == 0 && (n_done == 10 || n_done == 11)) hb_ffn_trace[role][n_done - 10][k] = clock64(); } while (0)
-#else
-#define TR(role, k) do { } while (0)
-#endif
 template <bool FUSE_O>
 __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid_constant__ CUtensorMap tmHhi,
                                                         const __grid_constant__ CUtensorMap tmHlo, const __grid_constant__ CUtensorMap tmW1hi,
                                                         const __grid_constant__ CUtensorMap tmW1lo, const __grid_constant__ CUtensorMap tmW2hi,
                                                         const __grid_constant__ CUtensorMap tmW2lo, const __grid_constant__ CUtensorMap tmWohi,
-                                                        const __grid_constant__ CUtensorMap tmWolo, const __grid_constant__ CUtensorMap tmOhi,
-                                                        const __grid_constant__ CUtensorMap tmOlo) {
+                                                        const __grid_constant__ CUtensorMap tmWolo) {
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
     uint8_t* sA1 = smem;                            // H tile: [kb][hi|lo][128 x 128 B]
     uint8_t* sA2 = sA1 + FFN_A_BYTES;               // relu(hidden chunk) tile, same layout
     uint8_t* ring = sA2 + FFN_A_BYTES;              // FFN_STAGES x FFN_RING_BYTES
-    __shared__ uint64_t full_bar[FFN_STAGES], empty_bar[FFN_STAGES], a1_full, a1_empty, f_full[2], f_empty[2], a2_full[2], a2_empty[2], a2_free,
-        o_full[2], o_empty[2], y_full, h_full;
-    __shared__ uint32_t tmem_base_s;
-    __shared__ uint32_t s_prog;  // tiles the producer lane has started (paces the L2 prefetch of the residual rows)
+    __shared__ uint64_t full_bar[FFN_STAGES], empty_bar[FFN_STAGES], a1_full, a1_empty;
     __shared__ __align__(16) float s_b1[512], s_b2[BN], s_lng[BN], s_lnb[BN], s_bo[BN], s_ln2g[BN], s_ln2b[BN];
-    __shared__ float s_red[2][2][BM], s_red2[2][2][BM];  // [slot][column half][row]: LayerNorm partial sums / squared deviations
-    __shared__ __align__(16) float s_stage[8][32 * 16];  // per-warp transpose buffers (see warp_store_f32x16)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        s_prog = 0;
-        for (int s = 0; s < FFN_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&a1_full, 1); mbar_init(&a1_empty, 1);
-        mbar_init(&y_full, 1); mbar_init(&h_full, G_EPI); mbar_init(&a2_free, 1);
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&f_full[a], 1); mbar_init(&f_empty[a], G_EPI);
-            mbar_init(&a2_full[a], G_EPI); mbar_init(&a2_empty[a], 1);  // per k-block of A2
-            mbar_init(&o_full[a], 1); mbar_init(&o_empty[a], G_EPI);
-        }
+        for (int s = 0; s < FFN_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C_THREADS); }
+        mbar_init(&a1_full, 1); mbar_init(&a1_empty, C_THREADS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = tid; i < 512; i += G_THREADS) s_b1[i] = g.b1[i];
     if (tid < BN) { s_b2[tid] = g.b2[tid]; s_lng[tid] = g.ln_g[tid]; s_lnb[tid] = g.ln_b[tid]; }
     if (FUSE_O && tid < BN) { s_bo[tid] = g.bo[tid]; s_ln2g[tid] = g.ln2_g[tid]; s_ln2b[tid] = g.ln2_b[tid]; }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
-    // TMEM columns: accF[0] 0..127, accF[1] 128..255, accO[0] 256..383, accO[1] 384..511 (FUSE_O: accO 256..383, X' 384..511)
 
     if (warp == G_PROD_WARP) {
         // =============================== producer: one lane issues the TMA copies ===============================
-        // The other lanes pull the residual rows E0 will add one tile from now towards L2 (fp32 X comes from DRAM: with 4
-        // dependent rounds of loads per thread, DRAM latency was 4.9 k cycles of E0 with the tensor pipe idle).
-        if (FUSE_O && lane != 0) {
-            uint32_t n = 0;
-            for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n++) {
-                while ((int)(n - atomicAdd(&s_prog, 0u)) > 1) __nanosleep(1000);  // at most one tile ahead of the tile lane 0 is loading
-                for (int i = lane - 1; i < BM * 4; i += 31) prefetch_l2((const char*)(g.X + (size_t)tile * BM * BN) + (size_t)i * 128);
-            }
-        }
         if (lane == 0) {
             uint32_t it_stage = 0, n_done = 0;
-            // H tile (resident for a whole tile): 2 k-blocks x (hi, lo).  Tile t+1's is requested as soon as F1(3) of tile t has
-            // released the buffer (behind the stages of step 6, whose ring slots F1(3) frees as well), not after the producer has
-            // queued all of tile t's weights: it is the first thing tile t+1 needs.
-            auto load_a1 = [&](uint32_t tile, uint32_t n) {
-                const int m0 = (int)(tile * BM);
-                mbar_wait(&a1_empty, (n & 1) ^ 1);
+            auto load_w = [&](const CUtensorMap* hi, const CUtensorMap* lo, int col, int row) {
+                const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
+                mbar_wait(&empty_bar[s], ph ^ 1);
+                const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
+                mbar_arrive_expect_tx(&full_bar[s], FFN_RING_BYTES);
+                tma_load_2d(sb, hi, &full_bar[s], col, row);
+                tma_load_2d(sb + BN * 128, lo, &full_bar[s], col, row);
+                it_stage++;
+            };
+            for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
+                // H (or O) tile, resident for the whole tile: 2 k-blocks x (hi, lo); free once F1(3) of the previous tile is done
+                mbar_wait(&a1_empty, (n_done & 1) ^ 1);
                 mbar_arrive_expect_tx(&a1_full, FFN_A_BYTES);
                 for (int kb = 0; kb < 2; kb++) {
-                    tma_load_2d(smem_u32(sA1) + kb * (2 * BM * 128), &tmHhi, &a1_full, kb * BK, m0);
-                    tma_load_2d(smem_u32(sA1) + kb * (2 * BM * 128) + BM * 128, &tmHlo, &a1_full, kb * BK, m0);
+                    tma_load_2d(smem_u32(sA1) + kb * (2 * BM * 128), &tmHhi, &a1_full, kb * BK, (int)(tile * BM));
+                    tma_load_2d(smem_u32(sA1) + kb * (2 * BM * 128) + BM * 128, &tmHlo, &a1_full, kb * BK, (int)(tile * BM));
                 }
-            };
-            if (blockIdx.x < g.m_tiles) load_a1(blockIdx.x, 0);
-            for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
-                atomicExch(&s_prog, n_done);  // (atomics: a progress flag polled by the other lanes, not a data hand-off)
-                if (FUSE_O) {  // Wo: 2 k-block tiles, ahead of the FFN weights
-                    for (int kb = 0; kb < 2; kb++, it_stage++) {
-                        const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
-                        mbar_wait(&empty_bar[s], ph ^ 1);
-                        const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
-                        mbar_arrive_expect_tx(&full_bar[s], FFN_RING_BYTES);
-                        tma_load_2d(sb, &tmWohi, &full_bar[s], kb * BK, 0);
-                        tma_load_2d(sb + BN * 128, &tmWolo, &full_bar[s], kb * BK, 0);
-                    }
-                }
-                // ---- the 16 weight k-block tiles of this tile, in MMA issue order
-                for (int st = 0; st < 8; st++) {
-                    int is2, c;
-                    ffn_step(st, is2, c);
-                    if (st == 7 && tile + gridDim.x < g.m_tiles) load_a1(tile + gridDim.x, n_done + 1);
-                    for (int kb = 0; kb < 2; kb++, it_stage++) {
-                        const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
-                        TR(2, 4 * st + 2 * kb);
-                        mbar_wait(&empty_bar[s], ph ^ 1);
-                        TR(2, 4 * st + 2 * kb + 1);
-                        const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
-                        mbar_arrive_expect_tx(&full_bar[s], FFN_RING_BYTES);
-                        // F1(c): rows = hidden units c*128.., K = C;   F2(c): rows = outputs, K-columns = hidden units c*128..
-                        const int crow = is2 ? 0 : c * 128, ccol = (is2 ? c * 128 : 0) + kb * BK;
-                        tma_load_2d(sb, is2 ? &tmW2hi : &tmW1hi, &full_bar[s], ccol, crow);
-                        tma_load_2d(sb + BN * 128, is2 ? &tmW2lo : &tmW1lo, &full_bar[s], ccol, crow);
-                    }
+                if (FUSE_O)
+                    for (int kb = 0; kb < 2; kb++) load_w(&tmWohi, &tmWolo, kb * BK, 0);
+                for (int c = 0; c < 4; c++) {
+                    // F1(c): rows = hidden units c*128.., K = C;   F2(c): rows = outputs, K-columns = hidden units c*128..
+                    for (int kb = 0; kb < 2; kb++) load_w(&tmW1hi, &tmW1lo, kb * BK, c * 128);
+                    for (int kb = 0; kb < 2; kb++) load_w(&tmW2hi, &tmW2lo, c * 128 + kb * BK, 0);
                 }
             }
         }
-    } else if (warp == G_MMA_WARP) {
-        // =============================== MMA issuer ===============================
-        if (lane == 0) {
-            uint32_t it_stage = 0, n_done = 0, nf[2] = {0, 0}, na2 = 0;  // na2: A2 k-block generations consumed
-            const uint32_t a1b = smem_u32(sA1), a2b = smem_u32(sA2);
-            for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
-                const uint32_t oacc = FUSE_O ? 0u : (n_done & 1);
-                TR(0, 0);
-                mbar_wait(&a1_full, n_done & 1);
-                TR(0, 1);
-                if (FUSE_O) {
-                    // ---- P0: accO = O · Wo^T (the previous tile's final epilogue must have drained accO)
-                    mbar_wait(&o_empty[0], (n_done & 1) ^ 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t tmem_d = tmem_base + 2 * BN;
-                    for (int kb = 0; kb < 2; kb++, it_stage++) {
-                        const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
-                        mbar_wait(&full_bar[s], ph);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
-                        const uint64_t dAh = make_desc(a1b + kb * (2 * BM * 128)), dAl = make_desc(a1b + kb * (2 * BM * 128) + BM * 128);
-                        const uint64_t dBh = make_desc(sb), dBl = make_desc(sb + BN * 128);
-#pragma unroll
-                        for (int k = 0; k < BK / 16; k++) {
-                            const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                            mma_bf16(tmem_d, dAh + adv, dBh + adv, (kb | k) ? 1u : 0u);
-                            mma_bf16(tmem_d, dAl + adv, dBh + adv, 1u);
-                            mma_bf16(tmem_d, dAh + adv, dBl + adv, 1u);
-                        }
-                        umma_commit(&empty_bar[s]);
-                    }
-                    umma_commit(&y_full);
-                    TR(0, 2);
-                    mbar_wait(&h_full, n_done & 1);
-                    TR(0, 3);  // E0 has replaced the O tile by H = LN2(X') in shared memory
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                }
-                for (int st = 0; st < 8; st++) {
-                    int is2, c;
-                    ffn_step(st, is2, c);
-                    uint32_t tmem_d, abase;
-                    TR(0, 4 + 4 * st);
-                    if (!is2) {
-                        const uint32_t j = c & 1;
-                        mbar_wait(&f_empty[j], (nf[j] & 1) ^ 1);  // epilogue has drained accF[j]
-                        tmem_d = tmem_base + j * BN;
-                        abase = a1b;
-                    } else {
-                        if (!FUSE_O && c == 0) mbar_wait(&o_empty[oacc], ((n_done >> 1) & 1) ^ 1);
-                        tmem_d = tmem_base + 2 * BN + oacc * BN;
-                        abase = a2b;
-                    }
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    TR(0, 5 + 4 * st);
-                    for (int kb = 0; kb < 2; kb++, it_stage++) {
-                        const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
-                        if (is2) mbar_wait(&a2_full[kb], na2 & 1);  // E1(c) has written this k-block of the hidden chunk
-                        mbar_wait(&full_bar[s], ph);
-                        TR(0, 6 + 4 * st + kb);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
-                        const uint64_t dAh = make_desc(abase + kb * (2 * BM * 128)), dAl = make_desc(abase + kb * (2 * BM * 128) + BM * 128);
-                        const uint64_t dBh = make_desc(sb), dBl = make_desc(sb + BN * 128);
-#pragma unroll
-                        for (int k = 0; k < BK / 16; k++) {
-                            const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                            const uint32_t accum = (is2 ? (c | kb | k) : (kb | k)) ? 1u : 0u;
-                            mma_bf16(tmem_d, dAh + adv, dBh + adv, accum);
-                            mma_bf16(tmem_d, dAl + adv, dBh + adv, 1u);
-                            mma_bf16(tmem_d, dAh + adv, dBl + adv, 1u);
-                        }
-                        umma_commit(&empty_bar[s]);
-                        if (is2) umma_commit(&a2_empty[kb]);      // E1(c+1) may refill this k-block while the other one is still being read
-                    }
-                    if (!is2) {
-                        umma_commit(&f_full[c & 1]);
-                        nf[c & 1]++;
-                        if (c == 3) umma_commit(&a1_empty);       // H tile no longer needed
-                    } else {
-                        na2++;
-                        if (c == 3) umma_commit(&o_full[oacc]);
-                    }
-                }
-            }
-        }
-    } else {
-        // =============================== epilogue: 8 warps, 64 columns each =======================
-        const int wq = warp & 3, eh = warp >> 2;  // TMEM lane quadrant, column half (= k-block of the A2 tile)
-        const int ch = eh * 64;
-        uint32_t n_done = 0, nf[2] = {0, 0}, na2 = 0;
-        for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
-            const uint32_t r = wq * 32 + lane;
-            const size_t row = (size_t)tile * BM + r;
-            if (!FUSE_O) {   // the residual rows this thread adds in the final epilogue (~10 us from now): start them towards L2
-                const float* pr = g.X + row * BN + ch;
-                prefetch_l2(pr); prefetch_l2(pr + 32);
-            }
-            if (FUSE_O) {
-                // ---- E0: X' = accO + bo + X (parked in TMEM), H = LN2(X') -> split bf16 -> over the O tile (A operand of FFN1)
-                float* stg = s_stage[warp];
-                const float* xblk = g.X + ((size_t)tile * BM + wq * 32) * BN + ch;
-                const uint32_t tacc = tmem_base + 2 * BN + ch + ((uint32_t)(wq * 32) << 16);
-                const uint32_t txs = tmem_base + 3 * BN + ch + ((uint32_t)(wq * 32) << 16);
-                float x[64];
-                if (g.x_blocked) {
-                    // tile-blocked residual stream (see FfnArgs::x_blocked): the row owner's 16 loads are coalesced as they are, all
-                    // of them in flight before the wait for the MMAs
-                    const float* xt = g.X + (size_t)tile * BM * BN + (size_t)(ch >> 2) * (BM * 4) + r * 4;
-                    if (tid == 0) TR(1, 50);
-#pragma unroll
-                    for (int q = 0; q < 16; q++) {
-                        const float4 t = *(const float4*)(xt + q * (BM * 4));
-                        x[4 * q] = t.x; x[4 * q + 1] = t.y; x[4 * q + 2] = t.z; x[4 * q + 3] = t.w;
-                    }
-                    if (tid == 0) TR(1, 0);
-                    mbar_wait(&y_full, n_done & 1);
-                    if (tid == 0) TR(1, 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                    for (int c0 = 0; c0 < 64; c0 += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(tacc + (uint32_t)c0, v);
-#pragma unroll
-                        for (int jj = 0; jj < 32; jj++) {
-                            x[c0 + jj] += __uint_as_float(v[jj]) + s_bo[ch + c0 + jj];
-                            v[jj] = __float_as_uint(x[c0 + jj]);
-                        }
-                        tmem_st32(txs + (uint32_t)c0, v);
-                    }
-                } else {
-                    float4 pre[2][4];
-                    warp_ldg_f32x16(lane, xblk, BN, pre[0]);       // requested before the wait for the MMAs, two blocks ahead
-                    warp_ldg_f32x16(lane, xblk + 16, BN, pre[1]);
-                    mbar_wait(&y_full, n_done & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                    for (int c0 = 0; c0 < 64; c0 += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(tacc + (uint32_t)c0, v);
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            float rv[16];
-                            warp_xpose_f32x16(stg, lane, pre[h], rv);
-                            if (c0 + h * 16 + 32 < 64) warp_ldg_f32x16(lane, xblk + c0 + h * 16 + 32, BN, pre[h]);
-#pragma unroll
-                            for (int jj = 0; jj < 16; jj++) {
-                                x[c0 + h * 16 + jj] = __uint_as_float(v[h * 16 + jj]) + s_bo[ch + c0 + h * 16 + jj] + rv[jj];
-                                v[h * 16 + jj] = __float_as_uint(x[c0 + h * 16 + jj]);
-                            }
-                        }
-                        tmem_st32(txs + (uint32_t)c0, v);
-                    }
-                }
-                if (tid == 0) TR(1, 44);
-                float sum = 0.f;
-#pragma unroll
-                for (int jj = 0; jj < 64; jj++) sum += x[jj];
-                s_red[0][eh][r] = sum;
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float mean = (s_red[0][0][r] + s_red[0][1][r]) * (1.f / BN);
-                float var = 0.f;
-#pragma unroll
-                for (int jj = 0; jj < 64; jj++) { const float d = x[jj] - mean; var = fmaf(d, d, var); }
-                s_red2[0][eh][r] = var;  // its own array: no barrier needed between the reads of the sums and this write
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float rstd = rsqrtf((s_red2[0][0][r] + s_red2[0][1][r]) * (1.f / BN) + 1e-5f);
-                if (tid == 0) TR(1, 45);
-                uint8_t* a1row = sA1 + (uint32_t)eh * (2 * BM * 128) + r * 128u;
-#pragma unroll
-                for (int q8 = 0; q8 < 8; q8++) {  // 8 x 8 channels = 8 x 16-byte chunks of hi and of lo
-                    uint32_t hi[4], lo[4];
-#pragma unroll
-                    for (int e = 0; e < 8; e += 2) {
-                        const int jj = q8 * 8 + e;
-                        const float a = (x[jj] - mean) * rstd * s_ln2g[ch + jj] + s_ln2b[ch + jj];
-                        const float bq = (x[jj + 1] - mean) * rstd * s_ln2g[ch + jj + 1] + s_ln2b[ch + jj + 1];
-                        split2(a, bq, hi[e >> 1], lo[e >> 1]);
-                    }
-                    const uint32_t off = (uint32_t)((q8 ^ (r & 7)) << 4);
-                    *(uint4*)(a1row + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                    *(uint4*)(a1row + BM * 128 + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of H -> tensor core
-                mbar_arrive(&h_full);
-                if (tid == 0) TR(1, 2);
-            }
-            for (int c = 0; c < 4; c++) {
-                // ---- E1(c): relu(accF + b1) -> split bf16 -> A2 (swizzled K-major), k-block by k-block: every thread does 32 hidden
-                //      units of k-block 0, hands it to the tensor pipe, then 32 of k-block 1 - so F2(c) starts after half of E1(c) and
-                //      E1(c+1) starts after half of F2(c) (one barrier pair per k-block; with one pair per chunk the two alternated)
-                const uint32_t j = c & 1;
-                if (tid == 0) TR(1, 3 + 4 * c);
-                mbar_wait(&f_full[j], nf[j] & 1);
-                nf[j]++;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (tid == 0) TR(1, 4 + 4 * c);
-                const uint32_t taddr = tmem_base + j * BN + eh * 32 + ((uint32_t)(wq * 32) << 16);
-                if (FUSE_O && c == 0) {
-                    // the previous tile's H tile (staged in A2 by its final epilogue) has been read by its TMA store: long done by
-                    // now, so the thread that owns the bulk group confirms it here and not on E0's critical path
-                    if (tid == 0) { tma_store_wait_read(); mbar_arrive(&a2_free); }
-                    mbar_wait(&a2_free, n_done & 1);
-                }
-#pragma unroll
-                for (int kb = 0; kb < 2; kb++) {
-                    mbar_wait(&a2_empty[kb], (na2 & 1) ^ 1);      // F2(c-1) has finished reading this k-block of A2
-                    if (tid == 0 && kb == 0) TR(1, 5 + 4 * c);
-                    uint8_t* a2row = sA2 + (uint32_t)kb * (2 * BM * 128) + r * 128u;
-                    uint32_t v[32];
-                    tmem_ld32(taddr + (uint32_t)(kb * 64), v);
-                    if (kb == 1) {  // accF[j] is drained
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                        mbar_arrive(&f_empty[j]);
-                    }
-                    const float* bb = s_b1 + c * 128 + kb * 64 + eh * 32;
-#pragma unroll
-                    for (int q8 = 0; q8 < 4; q8++) {              // 4 x 8 hidden units = 4 x 16-byte chunks of hi and of lo
-                        uint32_t hi[4], lo[4];
-#pragma unroll
-                        for (int e = 0; e < 8; e += 2)
-                            split2(fmaxf(__uint_as_float(v[q8 * 8 + e]) + bb[q8 * 8 + e], 0.f),
-                                   fmaxf(__uint_as_float(v[q8 * 8 + e + 1]) + bb[q8 * 8 + e + 1], 0.f), hi[e >> 1], lo[e >> 1]);
-                        const uint32_t off = (uint32_t)(((eh * 4 + q8) ^ (r & 7)) << 4);
-                        *(uint4*)(a2row + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                        *(uint4*)(a2row + BM * 128 + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of A2 -> tensor core
-                    mbar_arrive(&a2_full[kb]);
-                }
-                na2++;
-                if (tid == 0) TR(1, 6 + 4 * c);
-            }
-            // ---- final epilogue: X = accO + b2 + X ; LayerNorm -> split bf16 (partial sums exchanged between the halves)
-            const uint32_t oacc = FUSE_O ? 0u : (n_done & 1);
-            float4 pre[4];  // first residual block: requested before the wait for the last MMAs (it does not depend on them)
-            if (!FUSE_O) warp_ldg_f32x16(lane, g.X + ((size_t)tile * BM + wq * 32) * BN + ch, BN, pre);
-            if (tid == 0) TR(1, 40);
-            mbar_wait(&o_full[oacc], FUSE_O ? (n_done & 1) : ((n_done >> 1) & 1));
-            if (tid == 0) TR(1, 41);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem_base + 2 * BN + oacc * BN + ch + ((uint32_t)(wq * 32) << 16);
-            float x[64];
-            float* stg = s_stage[warp];
-            float* xblk = g.X + ((size_t)tile * BM + wq * 32) * BN + ch;  // this warp's [32 rows][64 cols] block of X
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(taddr + (uint32_t)c0, v);
-                if (FUSE_O) {  // the residual X' of this row was parked in TMEM by E0
-                    uint32_t xr[32];
-                    tmem_ld32(tmem_base + 3 * BN + ch + ((uint32_t)(wq * 32) << 16) + (uint32_t)c0, xr);
-#pragma unroll
-                    for (int jj = 0; jj < 32; jj++) x[c0 + jj] = __uint_as_float(v[jj]) + s_b2[ch + c0 + jj] + __uint_as_float(xr[jj]);
-                } else {
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        float rv[16];
-                        warp_xpose_f32x16(stg, lane, pre, rv);
-                        if (c0 + h * 16 + 16 < 64) warp_ldg_f32x16(lane, xblk + c0 + h * 16 + 16, BN, pre);
-#pragma unroll
-                        for (int jj = 0; jj < 16; jj++)
-                            x[c0 + h * 16 + jj] = __uint_as_float(v[h * 16 + jj]) + s_b2[ch + c0 + h * 16 + jj] + rv[jj];
-                        if (g.store_x) warp_store_f32x16(stg, lane, xblk + c0 + h * 16, BN, x + c0 + h * 16);
-                    }
-                }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&o_empty[oacc]);
-            if (tid == 0) TR(1, 42);
-            if (FUSE_O && g.store_x) {  // the residual stream is dead after the last layer: only its LayerNorm is consumed
-                if (g.x_blocked) {
-                    float* xt = g.X + (size_t)tile * BM * BN + (size_t)(ch >> 2) * (BM * 4) + r * 4;
-#pragma unroll
-                    for (int q = 0; q < 8; q++) *(float4*)(xt + q * (BM * 4)) = make_float4(x[4 * q], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]);
-                    // (chunks 8..15 go out between the LayerNorm steps below: the store path is the bottleneck here, ~190 cycles per
-                    //  warp-wide 512-byte store, and stalls the issuing warp unless there is arithmetic to overlap it with)
-                } else {
-#pragma unroll
-                    for (int c0 = 0; c0 < 64; c0 += 16) warp_store_f32x16(stg, lane, xblk + c0, BN, x + c0);
-                }
-            }
-            if (tid == 0) TR(1, 46);
-            float sum = 0.f;
-#pragma unroll
-            for (int jj = 0; jj < 64; jj++) sum += x[jj];
-            const uint32_t rs_ = FUSE_O ? 1u : oacc;  // E0 uses s_red[0]
-            s_red[rs_][eh][r] = sum;
-            asm volatile("bar.sync 2, 256;" ::: "memory");
-            const float mean = (s_red[rs_][0][r] + s_red[rs_][1][r]) * (1.f / BN);
-            float var = 0.f;
-#pragma unroll
-            for (int jj = 0; jj < 64; jj++) { const float d = x[jj] - mean; var = fmaf(d, d, var); }
-            s_red2[rs_][eh][r] = var;
-            asm volatile("bar.sync 2, 256;" ::: "memory");
-            const float rstd = rsqrtf((s_red2[rs_][0][r] + s_red2[rs_][1][r]) * (1.f / BN) + 1e-5f);
-            // LayerNorm(X) -> split bf16 -> the (idle) A2 tile in the layout of an operand tile ([kb][hi|lo][128 x 128 B], swizzled) ->
-            // 4 TMA stores by one thread.  (Row-owner -> coalesced transposes through the per-warp staging buffers, 16 STS/LDS/STG
-            // round trips per thread, were 5.8 k cycles of every tile during which nothing else could use the epilogue warps.)
-            if (tid == 0) TR(1, 47);
-            uint8_t* orow = sA2 + (uint32_t)eh * (2 * BM * 128) + r * 128u;
-#pragma unroll
-            for (int q8 = 0; q8 < 8; q8++) {
-                uint32_t hi[4], lo[4];
-#pragma unroll
-                for (int e = 0; e < 8; e += 2) {
-                    const int jj = q8 * 8 + e;
-                    const float a = (x[jj] - mean) * rstd * s_lng[ch + jj] + s_lnb[ch + jj];
-                    const float bq = (x[jj + 1] - mean) * rstd * s_lng[ch + jj + 1] + s_lnb[ch + jj + 1];
-                    split2(a, bq, hi[e >> 1], lo[e >> 1]);
-                }
-                const uint32_t off = (uint32_t)((q8 ^ (r & 7)) << 4);
-                *(uint4*)(orow + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                *(uint4*)(orow + BM * 128 + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                if (FUSE_O && g.store_x && g.x_blocked) {
-                    float* xt = g.X + (size_t)tile * BM * BN + (size_t)(ch >> 2) * (BM * 4) + r * 4;
-                    const int q = 8 + q8;
-                    *(float4*)(xt + q * (BM * 4)) = make_float4(x[4 * q], x[4 * q + 1], x[4 * q + 2], x[4 * q + 3]);
-                }
-            }
-            if (tid == 0) TR(1, 48);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("bar.sync 2, 256;" ::: "memory");
-            if (tid == 0) TR(1, 49);
-            if (tid == 0) {
-                const int m0 = (int)(tile * BM);
-                for (int kb = 0; kb < 2; kb++) {
-                    tma_store_2d(&tmOhi, smem_u32(sA2) + kb * (2 * BM * 128), kb * BK, m0);
-                    tma_store_2d(&tmOlo, smem_u32(sA2) + kb * (2 * BM * 128) + BM * 128, kb * BK, m0);
-                }
-                tma_store_commit();
-                if (!FUSE_O) tma_store_wait_read();  // no E0 in front of the next E1(0): wait here
-            }
-            if (!FUSE_O) asm volatile("bar.sync 2, 256;" ::: "memory");
-            if (tid == 0) TR(1, 43);
-        }
+        return;
     }
-    if (tid == 0) tma_store_wait_all();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+    // =============================== consumers ===============================
+    const int wg = warp >> 2;
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), fc = (lane & 3) * 2;
+    const uint32_t a1b = smem_u32(sA1) + wg * 64 * 128, a2b = smem_u32(sA2) + wg * 64 * 128;  // this warpgroup's rows
+    uint32_t it_stage = 0, n_done = 0;
+    float accO[64], accF[64];
+    // two k-blocks of A (resident tile at abase) against the next two ring stages
+    auto contract = [&](float (&acc)[64], uint32_t abase, bool zero) {
+        for (int kb = 0; kb < 2; kb++, it_stage++) {
+            const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
+            const uint32_t a = abase + kb * (2 * BM * 128);
+            mma_kblock(acc, a, a + BM * 128, sb, sb + BN * 128, zero && kb == 0);
+        }
+        wg_wait<0>();
+        acc_fence(acc);
+        mbar_arrive(&empty_bar[(it_stage - 2) % FFN_STAGES]);
+        mbar_arrive(&empty_bar[(it_stage - 1) % FFN_STAGES]);
+    };
+    for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
+        const size_t row0 = (size_t)tile * BM + fr;
+        if (!FUSE_O) {  // accO = X + b2: the FFN2 contractions accumulate on top of the residual row
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int c = 8 * j + fc;
+                const float2 x0 = *(const float2*)(g.X + row0 * BN + c), x1 = *(const float2*)(g.X + (row0 + 8) * BN + c);
+                accO[4 * j] = x0.x + s_b2[c]; accO[4 * j + 1] = x0.y + s_b2[c + 1];
+                accO[4 * j + 2] = x1.x + s_b2[c]; accO[4 * j + 3] = x1.y + s_b2[c + 1];
+            }
+        }
+        mbar_wait(&a1_full, n_done & 1);
+        if (FUSE_O) {
+            // ---- P0 + E0: X' = O · Wo^T + bo + X;  H = LN2(X') over this warpgroup's rows of the O tile
+            contract(accO, a1b, true);
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int c = 8 * j + fc;
+                const float2 x0 = *(const float2*)(g.X + row0 * BN + c), x1 = *(const float2*)(g.X + (row0 + 8) * BN + c);
+                accO[4 * j] = accO[4 * j] + s_bo[c] + x0.x; accO[4 * j + 1] = accO[4 * j + 1] + s_bo[c + 1] + x0.y;
+                accO[4 * j + 2] = accO[4 * j + 2] + s_bo[c] + x1.x; accO[4 * j + 3] = accO[4 * j + 3] + s_bo[c + 1] + x1.y;
+            }
+            float ln[4];
+            frag_ln_stats(accO, ln[0], ln[1], ln[2], ln[3]);
+            bar_sync(1 + wg, 128);  // every warp of the warpgroup is past P0 before its O rows are overwritten
+            frag_store_tile(accO, sA1, fr, fc, s_ln2g, s_ln2b, ln);
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int c = 8 * j + fc;
+                accO[4 * j] += s_b2[c]; accO[4 * j + 1] += s_b2[c + 1]; accO[4 * j + 2] += s_b2[c]; accO[4 * j + 3] += s_b2[c + 1];
+            }
+            fence_async_smem();
+            bar_sync(1 + wg, 128);  // the warpgroup's H rows are complete before its FFN1 reads them
+        }
+        for (int c = 0; c < 4; c++) {
+            contract(accF, a1b, true);                                 // F1(c)
+            if (c == 3) mbar_arrive(&a1_empty);                        // the H tile is no longer needed
+#pragma unroll
+            for (int j = 0; j < 16; j++) {                             // E1(c)
+                const float b0 = s_b1[c * 128 + 8 * j + fc], b1 = s_b1[c * 128 + 8 * j + fc + 1];
+                accF[4 * j] = fmaxf(accF[4 * j] + b0, 0.f); accF[4 * j + 1] = fmaxf(accF[4 * j + 1] + b1, 0.f);
+                accF[4 * j + 2] = fmaxf(accF[4 * j + 2] + b0, 0.f); accF[4 * j + 3] = fmaxf(accF[4 * j + 3] + b1, 0.f);
+            }
+            frag_store_tile(accF, sA2, fr, fc);
+            fence_async_smem();
+            bar_sync(1 + wg, 128);
+            contract(accO, a2b, false);                                // F2(c)
+            bar_sync(1 + wg, 128);                                     // F2(c) has read A2 before the next E1 overwrites it
+        }
+        // ---- final epilogue: X = accO (residual already in); LayerNorm -> split bf16
+        if (g.store_x) frag_store_f32(accO, g.X, BN, row0, 0, fc);
+        frag_layernorm(accO, s_lng, s_lnb, fc);
+        frag_store_split(accO, g.out_hi, g.out_lo, BN, row0, 0, fc);
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Fused QKV projection + read-axis attention for C == 128, 4 heads of 32:
-//   per 128-token tile (4 positions x 32 read tokens) and head h:
-//     MMA(h):  acc[h][128 x 96] = H_tile · Wp[h]^T      Wp[h] = [Wq_h ; Wk_h ; Wv_h] (rows permuted at load), tcgen05
-//     ATT(h):  the warp that owns a position's 32 TMEM lanes reads q|k|v of its 32 tokens (lane = token) and runs the
-//              position's 32x32 attention entirely inside the warp: q, k, v are parked as split-bf16 rows in the warp's
-//              private shared-memory block, S = q·k^T and O = P·v run as warp-level mma.sync.m16n8k16 (operands by
-//              ldmatrix, bf16x3 like every other contraction here), softmax on the accumulator fragments in registers.
-//   tcgen05 cannot take these: its smallest M is 64 rows of ONE operand pair, but every 32-token position has its own
-//   K and V (a 128-row tile would be a block-diagonal product, 4x wasted, with P and V^T staged through shared memory);
-//   a first version with fp32 FFMA dot products out of shared memory was bound by the LSU (a broadcast LDS.128 costs two
-//   wavefronts per 4 FMAs per lane: 73 % of the shared-memory pipe, 2.4 ms per step) — ncu: profiles/r01d_*.
-//   The two compute warpgroups take alternate heads; the four heads have their own TMEM accumulators, so the MMAs and
-//   weight traffic run a whole tile ahead of the attention.  q, k, v never reach HBM: saves writing and re-reading the
-//   fp32 [T, 3C] tensor (3 KB per token and layer) and one kernel's fill/drain.
+//   per 128-token tile (4 positions x 32 read tokens) and head h, consumer warpgroup wg (positions 2 wg, 2 wg + 1):
+//     MMA(h):  acc[64 x 96] = H rows · Wp[h]^T      Wp[h] = [Wq_h ; Wk_h ; Wv_h] (rows permuted at load), wgmma
+//     ATT(h):  the warps write q|k|v (+ bias, q scaled) of their rows as split bf16 into the position's shared-memory arrays;
+//              the two warps of a position then take 16 queries each: S = q·k^T and O = P·v as warp-level
+//              mma.sync.m16n8k16 (operands by ldmatrix, bf16x3 like every other contraction here), softmax on the
+//              accumulator fragments in registers.
+//   wgmma cannot take the attention itself: every 32-token position has its own K and V, so a 64-row tile would be a
+//   block-diagonal product.  q, k, v never reach HBM: saves writing and re-reading the fp32 [T, 3C] tensor.
 // ------------------------------------------------------------------------------------------------
 constexpr int QA_HROWS = 96;                        // q|k|v rows of one head
 constexpr int QA_RING_BYTES = 2 * QA_HROWS * 128;   // one k-block of a head's weights, hi + lo: 24 KB
 constexpr int QA_STAGES = 3;
-constexpr int QA_WARP_BYTES = 8192;                 // per compute warp: 4 swizzled [32 rows][64 B] bf16 arrays
-constexpr uint32_t IDESC_N96 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(QA_HROWS >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+constexpr int QA_POS_BYTES = 6 * 2048;              // per position: q, k, v as swizzled [32 rows][64 B] hi and lo arrays
 
-__device__ __forceinline__ void mma_bf16_n96(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(IDESC_N96), "r"(accumulate)
-        : "memory");
-}
-// single-lane waits of the producer / MMA warps: back off between polls so the spinning does not take issue slots
-// from the compute warps that share the scheduler
-__device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity) {
-    uint32_t done;
-    for (;;) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if (done) break;
-        __nanosleep(64);
-    }
-}
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
@@ -980,30 +496,10 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// [32 rows][32 bf16] array with 64-byte rows; the 16-byte chunk c of row r lives at chunk c ^ ((r >> 1) & 3), which makes the
-// row-owner 16-byte stores, the ldmatrix row fetches (8 rows, same chunk) and the staged output rows all bank-conflict free
+// [32 rows][32 bf16] array with 64-byte rows; the 16-byte chunk c of row r lives at chunk c ^ ((r >> 1) & 3), which keeps the
+// ldmatrix row fetches (8 rows, same chunk) and the staged output rows bank-conflict free
 __device__ __forceinline__ uint32_t qa_off(int row, int chunk) { return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4)); }
-// the lane's row of 32 fp32 values (TMEM words + bias, scaled) -> split bf16 -> its row of the hi and lo arrays
-__device__ __forceinline__ void qa_store_row(uint8_t* hi_arr, uint8_t* lo_arr, int lane, const uint32_t (&v)[32], const float* bias, float scale) {
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int e = 0; e < 8; e += 2)
-            split2((__uint_as_float(v[c * 8 + e]) + bias[c * 8 + e]) * scale, (__uint_as_float(v[c * 8 + e + 1]) + bias[c * 8 + e + 1]) * scale,
-                   hi[e >> 1], lo[e >> 1]);
-        const uint32_t off = qa_off(lane, c);
-        *(uint4*)(hi_arr + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *(uint4*)(lo_arr + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    }
-}
 
-#ifdef HB_FFN_TRACE
-__device__ unsigned long long hb_qa_trace[3][2][64];  // [role: 0 MMA, 1 compute thread 0, 2 compute warp 4 lane 0][tile 10/11][event]
-#define TQ(role, k) do { if (blockIdx.x == 0 && (n_done == 10 || n_done == 11)) hb_qa_trace[role][n_done - 10][k] = clock64(); } while (0)
-#else
-#define TQ(role, k) do { } while (0)
-#endif
 __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, const __grid_constant__ CUtensorMap tmHhi,
                                                              const __grid_constant__ CUtensorMap tmHlo, const __grid_constant__ CUtensorMap tmWhi,
                                                              const __grid_constant__ CUtensorMap tmWlo) {
@@ -1011,35 +507,25 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, con
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
     uint8_t* sA = smem;                                   // H tile: [kb][hi|lo][128 x 128 B]
     uint8_t* ring = sA + FFN_A_BYTES;                     // QA_STAGES x QA_RING_BYTES
-    uint8_t* sW = ring + QA_STAGES * QA_RING_BYTES;       // [8 warps][QA_WARP_BYTES]
-    __shared__ uint64_t full_bar[QA_STAGES], empty_bar[QA_STAGES], a_full, a_empty, h_full[4], h_empty[4];
-    __shared__ uint32_t tmem_base_s;
+    uint8_t* sP = ring + QA_STAGES * QA_RING_BYTES;       // [4 positions][QA_POS_BYTES]
+    __shared__ uint64_t full_bar[QA_STAGES], empty_bar[QA_STAGES], a_full, a_empty;
     __shared__ __align__(16) float s_bias[4 * QA_HROWS];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        for (int s = 0; s < QA_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&a_full, 1); mbar_init(&a_empty, 1);
-        for (int a = 0; a < 4; a++) { mbar_init(&h_full[a], 1); mbar_init(&h_empty[a], G_EPI / 2); }
+        for (int s = 0; s < QA_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], C_THREADS); }
+        mbar_init(&a_full, 1); mbar_init(&a_empty, C_THREADS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = tid; i < 4 * QA_HROWS; i += G_THREADS) s_bias[i] = g.bias[i];
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
-    // TMEM columns: head h accumulates in [h*128, h*128 + 96)
 
     if (warp == G_PROD_WARP) {
         if (lane == 0) {
             uint32_t it_stage = 0, n_done = 0;
             for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
                 const int m0 = (int)(tile * BM);
-                mbar_wait_sleep(&a_empty, (n_done & 1) ^ 1);
+                mbar_wait(&a_empty, (n_done & 1) ^ 1);
                 mbar_arrive_expect_tx(&a_full, FFN_A_BYTES);
                 for (int kb = 0; kb < 2; kb++) {
                     tma_load_2d(smem_u32(sA) + kb * (2 * BM * 128), &tmHhi, &a_full, kb * BK, m0);
@@ -1048,7 +534,7 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, con
                 for (int h = 0; h < 4; h++)
                     for (int kb = 0; kb < 2; kb++, it_stage++) {
                         const uint32_t s = it_stage % QA_STAGES, ph = (it_stage / QA_STAGES) & 1;
-                        mbar_wait_sleep(&empty_bar[s], ph ^ 1);
+                        mbar_wait(&empty_bar[s], ph ^ 1);
                         const uint32_t sb = smem_u32(ring + (size_t)s * QA_RING_BYTES);
                         mbar_arrive_expect_tx(&full_bar[s], QA_RING_BYTES);
                         tma_load_2d(sb, &tmWhi, &full_bar[s], kb * BK, h * QA_HROWS);
@@ -1056,215 +542,172 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, con
                     }
             }
         }
-    } else if (warp == G_MMA_WARP) {
-        if (lane == 0) {
-            uint32_t it_stage = 0, n_done = 0;
-            const uint32_t ab = smem_u32(sA);
-            for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
-                TQ(0, 0);
-                mbar_wait_sleep(&a_full, n_done & 1);
-                TQ(0, 1);
-                for (int h = 0; h < 4; h++) {
-                    TQ(0, 2 + 4 * h);
-                    mbar_wait_sleep(&h_empty[h], (n_done & 1) ^ 1);  // the previous tile's head h has been read out of this accumulator
-                    TQ(0, 3 + 4 * h);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t tmem_d = tmem_base + h * BN;
-                    for (int kb = 0; kb < 2; kb++, it_stage++) {
-                        const uint32_t s = it_stage % QA_STAGES, ph = (it_stage / QA_STAGES) & 1;
-                        mbar_wait_sleep(&full_bar[s], ph);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sb = smem_u32(ring + (size_t)s * QA_RING_BYTES);
-                        const uint64_t dAh = make_desc(ab + kb * (2 * BM * 128)), dAl = make_desc(ab + kb * (2 * BM * 128) + BM * 128);
-                        const uint64_t dBh = make_desc(sb), dBl = make_desc(sb + QA_HROWS * 128);
+        return;
+    }
+    // =============================== consumers ===============================
+    const int wg = warp >> 2;
+    const int pos = wg * 2 + ((warp & 3) >> 1);     // position of the tile whose rows this warp holds
+    const int mt = warp & 1;                        // this warp's 16 tokens of the position: rows mt*16 .. mt*16+15
+    const int gq = lane >> 2, tq = lane & 3;        // mma fragment coordinates: row group, column pair
+    uint8_t* pb = sP + (size_t)pos * QA_POS_BYTES;
+    uint8_t *aQh = pb, *aQl = pb + 2048, *aKh = pb + 4096, *aKl = pb + 6144, *aVh = pb + 8192, *aVl = pb + 10240;
+    const uint32_t uQh = smem_u32(aQh), uQl = smem_u32(aQl), uKh = smem_u32(aKh), uKl = smem_u32(aKl), uVh = smem_u32(aVh),
+                   uVl = smem_u32(aVl);
+    const float scale_l2 = rsqrtf(32.f) * 1.4426950408889634f;  // 1/sqrt(dh) and log2(e): scores come out in the exp2 domain
+    const uint32_t ab = smem_u32(sA) + wg * 64 * 128;
+    uint32_t it_stage = 0, n_done = 0;
+    for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
+        mbar_wait(&a_full, n_done & 1);
+        for (int h = 0; h < 4; h++) {
+            float acc[48];
+            for (int kb = 0; kb < 2; kb++, it_stage++) {
+                const uint32_t s = it_stage % QA_STAGES, ph = (it_stage / QA_STAGES) & 1;
+                mbar_wait(&full_bar[s], ph);
+                const uint32_t sb = smem_u32(ring + (size_t)s * QA_RING_BYTES);
+                const uint32_t a = ab + kb * (2 * BM * 128);
+                const uint64_t dAh = make_desc(a), dAl = make_desc(a + BM * 128), dBh = make_desc(sb), dBl = make_desc(sb + QA_HROWS * 128);
+                wg_fence();
 #pragma unroll
-                        for (int k = 0; k < BK / 16; k++) {
-                            const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                            mma_bf16_n96(tmem_d, dAh + adv, dBh + adv, (kb | k) ? 1u : 0u);
-                            mma_bf16_n96(tmem_d, dAl + adv, dBh + adv, 1u);
-                            mma_bf16_n96(tmem_d, dAh + adv, dBl + adv, 1u);
-                        }
-                        umma_commit(&empty_bar[s]);
-                    }
-                    umma_commit(&h_full[h]);
-                    TQ(0, 4 + 4 * h);
+                for (int k = 0; k < BK / 16; k++) {
+                    const uint64_t adv = (uint64_t)(k * 2);
+                    wgmma_n96(acc, dAh + adv, dBh + adv, (kb | k) ? 1u : 0u);
+                    wgmma_n96(acc, dAl + adv, dBh + adv, 1u);
+                    wgmma_n96(acc, dAh + adv, dBl + adv, 1u);
                 }
-                umma_commit(&a_empty);  // H tile no longer needed
+                wg_commit();
             }
-        }
-    } else {
-        // =============================== attention: 8 warps; warp & 3 = position of the tile, warp >> 2 = head parity ====
-        const int wq = warp & 3, wg = warp >> 2;
-        const int gq = lane >> 2, tq = lane & 3;   // mma fragment coordinates: row group, column pair
-        uint8_t* wb = sW + (size_t)warp * QA_WARP_BYTES;
-        uint8_t *aQh = wb, *aQl = wb + 2048, *aKh = wb + 4096, *aKl = wb + 6144;  // V (hi, lo) reuses the Q arrays, the output staging the K arrays
-        const uint32_t uQh = smem_u32(aQh), uQl = smem_u32(aQl), uKh = smem_u32(aKh), uKl = smem_u32(aKl);
-        const float scale_l2 = rsqrtf(32.f) * 1.4426950408889634f;  // 1/sqrt(dh) and log2(e): scores come out in the exp2 domain
-        uint32_t n_done = 0;
-        for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
-            for (int hh = 0; hh < 2; hh++) {
-                const int h = hh * 2 + wg;
-                const int trole = 1 + wg;
-                if (lane == 0 && wq == 0) TQ(trole, 0 + 10 * hh);
-                mbar_wait(&h_full[h], n_done & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0 && wq == 0) TQ(trole, 1 + 10 * hh);
-                const uint32_t taddr = tmem_base + h * BN + ((uint32_t)(wq * 32) << 16);
-                const float* bb = s_bias + h * QA_HROWS;
-                {
-                    uint32_t v[32];
-                    tmem_ld32(taddr, v);        // q of this lane's token
-                    qa_store_row(aQh, aQl, lane, v, bb, scale_l2);
-                    tmem_ld32(taddr + 32, v);   // k
-                    qa_store_row(aKh, aKl, lane, v, bb + 32, 1.f);
+            wg_wait<0>();
+            acc_fence(acc);
+            mbar_arrive(&empty_bar[(it_stage - 2) % QA_STAGES]);
+            mbar_arrive(&empty_bar[(it_stage - 1) % QA_STAGES]);
+            if (h == 3) mbar_arrive(&a_empty);  // H tile no longer needed
+            // ---- q|k|v of this warp's rows -> split bf16 -> the position's arrays (the partner warp is done with head h-1's)
+            bar_sync(3 + pos, 64);
+            const float* bb = s_bias + h * QA_HROWS;
+#pragma unroll
+            for (int j = 0; j < 12; j++) {
+                const int c = 8 * j + 2 * tq;                  // column of q|k|v
+                const float sc = j < 4 ? scale_l2 : 1.f;
+                uint8_t* hi_arr = j < 4 ? aQh : (j < 8 ? aKh : aVh);
+                const int cc = c & 31;
+#pragma unroll
+                for (int hf = 0; hf < 2; hf++) {
+                    const int row = mt * 16 + hf * 8 + gq;     // token of the position
+                    uint32_t hw, lw;
+                    split2((acc[4 * j + 2 * hf] + bb[c]) * sc, (acc[4 * j + 2 * hf + 1] + bb[c + 1]) * sc, hw, lw);
+                    const uint32_t off = qa_off(row, cc >> 3) + (cc & 7) * 2;
+                    *(uint32_t*)(hi_arr + off) = hw;
+                    *(uint32_t*)(hi_arr + 2048 + off) = lw;
                 }
-                __syncwarp();
-                if (lane == 0 && wq == 0) TQ(trole, 2 + 10 * hh);
-                // ---- S = q·k^T: [32 queries][32 keys] as 2 x 4 accumulator tiles of m16n8
-                float sacc[2][4][4];
+            }
+            bar_sync(3 + pos, 64);
+            // ---- S = q·k^T: [16 queries][32 keys] as 4 accumulator tiles of m16n8
+            float sacc[4][4];
 #pragma unroll
-                for (int mt = 0; mt < 2; mt++)
+            for (int nt = 0; nt < 4; nt++)
 #pragma unroll
-                    for (int nt = 0; nt < 4; nt++)
-#pragma unroll
-                        for (int e = 0; e < 4; e++) sacc[mt][nt][e] = 0.f;
-                {
-                    uint32_t qh[2][2][4], ql[2][2][4];
-#pragma unroll
-                    for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-                        for (int ks = 0; ks < 2; ks++) {
-                            const uint32_t off = qa_off(mt * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, ks * 2 + (lane >> 4));
-                            ldsm_x4(uQh + off, qh[mt][ks]);
-                            ldsm_x4(uQl + off, ql[mt][ks]);
-                        }
-#pragma unroll
-                    for (int ntp = 0; ntp < 2; ntp++)
-#pragma unroll
-                        for (int ks = 0; ks < 2; ks++) {
-                            uint32_t kh[4], kl[4];
-                            const uint32_t off = qa_off(ntp * 16 + (lane & 7) + (lane >> 4) * 8, ks * 2 + ((lane >> 3) & 1));
-                            ldsm_x4(uKh + off, kh);
-                            ldsm_x4(uKl + off, kl);
-#pragma unroll
-                            for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-                                for (int j = 0; j < 2; j++) {
-                                    mma16816(sacc[mt][ntp * 2 + j], qh[mt][ks], kh[2 * j], kh[2 * j + 1]);
-                                    mma16816(sacc[mt][ntp * 2 + j], ql[mt][ks], kh[2 * j], kh[2 * j + 1]);
-                                    mma16816(sacc[mt][ntp * 2 + j], qh[mt][ks], kl[2 * j], kl[2 * j + 1]);
-                                }
-                        }
-                }
-                if (lane == 0 && wq == 0) TQ(trole, 3 + 10 * hh);
-                // ---- softmax over the 31 real keys (key 31 is the pad token).  A lane holds, for each of its 4 query rows
-                //      (gq + 8*i), the 8 keys {8*nt + 2*tq, +1}; the other 24 keys of a row are in the 3 neighbouring lanes.
-                float inv[2][2];
-#pragma unroll
-                for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-                    for (int hf = 0; hf < 2; hf++) {
-                        if (tq == 3) sacc[mt][3][2 * hf + 1] = -INFINITY;
-                        float m = -INFINITY;
-#pragma unroll
-                        for (int nt = 0; nt < 4; nt++) m = fmaxf(m, fmaxf(sacc[mt][nt][2 * hf], sacc[mt][nt][2 * hf + 1]));
-                        m = fmaxf(m, __shfl_xor_sync(HB_FULL, m, 1));
-                        m = fmaxf(m, __shfl_xor_sync(HB_FULL, m, 2));
-                        float l = 0.f;
-#pragma unroll
-                        for (int nt = 0; nt < 4; nt++) {
-                            const float p0 = exp2f(sacc[mt][nt][2 * hf] - m), p1 = exp2f(sacc[mt][nt][2 * hf + 1] - m);
-                            sacc[mt][nt][2 * hf] = p0; sacc[mt][nt][2 * hf + 1] = p1;
-                            l += p0 + p1;
-                        }
-                        l += __shfl_xor_sync(HB_FULL, l, 1);
-                        l += __shfl_xor_sync(HB_FULL, l, 2);
-                        const int row = mt * 16 + hf * 8 + gq;
-                        inv[mt][hf] = (row < R_COLS) ? 1.f / l : 0.f;  // the pad token's output row is written as zeros
-                    }
-                if (lane == 0 && wq == 0) TQ(trole, 4 + 10 * hh);
-                // ---- v: read it out of TMEM only now (the Q arrays are free once every lane has its fragments)
-                __syncwarp();
-                {
-                    uint32_t v[32];
-                    tmem_ld32(taddr + 64, v);
-                    qa_store_row(aQh, aQl, lane, v, bb + 64, 1.f);
-                }
-                // the accumulator is drained: the MMAs of the next tile's head h may overwrite it
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(&h_empty[h]);
-                __syncwarp();
-                if (lane == 0 && wq == 0) TQ(trole, 5 + 10 * hh);
-                // ---- O = P·v: P fragments come straight from the S accumulator layout (two n-tiles = one k16 A fragment)
-                float oacc[2][4][4];
-#pragma unroll
-                for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-                    for (int dt = 0; dt < 4; dt++)
-#pragma unroll
-                        for (int e = 0; e < 4; e++) oacc[mt][dt][e] = 0.f;
+                for (int e = 0; e < 4; e++) sacc[nt][e] = 0.f;
+            {
+                uint32_t qh[2][4], ql[2][4];
 #pragma unroll
                 for (int ks = 0; ks < 2; ks++) {
-                    uint32_t ph[2][4], pl[2][4];
-#pragma unroll
-                    for (int mt = 0; mt < 2; mt++) {
-                        split2(sacc[mt][2 * ks][0], sacc[mt][2 * ks][1], ph[mt][0], pl[mt][0]);
-                        split2(sacc[mt][2 * ks][2], sacc[mt][2 * ks][3], ph[mt][1], pl[mt][1]);
-                        split2(sacc[mt][2 * ks + 1][0], sacc[mt][2 * ks + 1][1], ph[mt][2], pl[mt][2]);
-                        split2(sacc[mt][2 * ks + 1][2], sacc[mt][2 * ks + 1][3], ph[mt][3], pl[mt][3]);
-                    }
-#pragma unroll
-                    for (int dp = 0; dp < 2; dp++) {
-                        uint32_t vh[4], vl[4];
-                        const uint32_t off = qa_off(ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dp * 2 + (lane >> 4));
-                        ldsm_x4_trans(uQh + off, vh);
-                        ldsm_x4_trans(uQl + off, vl);
-#pragma unroll
-                        for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-                            for (int j = 0; j < 2; j++) {
-                                mma16816(oacc[mt][dp * 2 + j], ph[mt], vh[2 * j], vh[2 * j + 1]);
-                                mma16816(oacc[mt][dp * 2 + j], pl[mt], vh[2 * j], vh[2 * j + 1]);
-                                mma16816(oacc[mt][dp * 2 + j], ph[mt], vl[2 * j], vl[2 * j + 1]);
-                            }
-                    }
+                    const uint32_t off = qa_off(mt * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, ks * 2 + (lane >> 4));
+                    ldsm_x4(uQh + off, qh[ks]);
+                    ldsm_x4(uQl + off, ql[ks]);
                 }
-                if (lane == 0 && wq == 0) TQ(trole, 6 + 10 * hh);
-                // ---- normalise, split, stage the 32 output rows (64 B of hi and of lo each) in the K arrays, store coalesced
-                uint32_t* sth = (uint32_t*)aKh;
-                uint32_t* stl = (uint32_t*)aKl;
 #pragma unroll
-                for (int mt = 0; mt < 2; mt++)
+                for (int ntp = 0; ntp < 2; ntp++)
 #pragma unroll
-                    for (int hf = 0; hf < 2; hf++) {
-                        const int row = mt * 16 + hf * 8 + gq;
+                    for (int ks = 0; ks < 2; ks++) {
+                        uint32_t kh[4], kl[4];
+                        const uint32_t off = qa_off(ntp * 16 + (lane & 7) + (lane >> 4) * 8, ks * 2 + ((lane >> 3) & 1));
+                        ldsm_x4(uKh + off, kh);
+                        ldsm_x4(uKl + off, kl);
 #pragma unroll
-                        for (int dt = 0; dt < 4; dt++) {
-                            uint32_t hi, lo;
-                            split2(oacc[mt][dt][2 * hf] * inv[mt][hf], oacc[mt][dt][2 * hf + 1] * inv[mt][hf], hi, lo);
-                            const int w = row * 16 + ((dt ^ ((row >> 1) & 3)) << 2) + tq;
-                            sth[w] = hi;
-                            stl[w] = lo;
+                        for (int j = 0; j < 2; j++) {
+                            mma16816(sacc[ntp * 2 + j], qh[ks], kh[2 * j], kh[2 * j + 1]);
+                            mma16816(sacc[ntp * 2 + j], ql[ks], kh[2 * j], kh[2 * j + 1]);
+                            mma16816(sacc[ntp * 2 + j], qh[ks], kl[2 * j], kl[2 * j + 1]);
                         }
                     }
-                __syncwarp();
-                const size_t rb = ((size_t)tile * BM + wq * 32) * BN + h * 32;  // row 0 of this position, this head's columns
-#pragma unroll
-                for (int jj = 0; jj < 4; jj++) {
-                    const int rr = jj * 8 + (lane >> 2), cq = lane & 3;
-                    const int w = rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2);
-                    *(uint4*)(g.out_hi + rb + (size_t)rr * BN + cq * 8) = *(const uint4*)(sth + w);
-                    *(uint4*)(g.out_lo + rb + (size_t)rr * BN + cq * 8) = *(const uint4*)(stl + w);
-                }
-                __syncwarp();
-                if (lane == 0 && wq == 0) TQ(trole, 7 + 10 * hh);
             }
+            // ---- softmax over the 31 real keys (key 31 is the pad token).  A lane holds, for each of its 2 query rows
+            //      (gq + 8*hf), the 8 keys {8*nt + 2*tq, +1}; the other 24 keys of a row are in the 3 neighbouring lanes.
+            float inv[2];
+#pragma unroll
+            for (int hf = 0; hf < 2; hf++) {
+                if (tq == 3) sacc[3][2 * hf + 1] = -INFINITY;
+                float m = -INFINITY;
+#pragma unroll
+                for (int nt = 0; nt < 4; nt++) m = fmaxf(m, fmaxf(sacc[nt][2 * hf], sacc[nt][2 * hf + 1]));
+                m = fmaxf(m, __shfl_xor_sync(HB_FULL, m, 1));
+                m = fmaxf(m, __shfl_xor_sync(HB_FULL, m, 2));
+                float l = 0.f;
+#pragma unroll
+                for (int nt = 0; nt < 4; nt++) {
+                    const float p0 = exp2f(sacc[nt][2 * hf] - m), p1 = exp2f(sacc[nt][2 * hf + 1] - m);
+                    sacc[nt][2 * hf] = p0; sacc[nt][2 * hf + 1] = p1;
+                    l += p0 + p1;
+                }
+                l += __shfl_xor_sync(HB_FULL, l, 1);
+                l += __shfl_xor_sync(HB_FULL, l, 2);
+                const int row = mt * 16 + hf * 8 + gq;
+                inv[hf] = (row < R_COLS) ? 1.f / l : 0.f;  // the pad token's output row is written as zeros
+            }
+            // ---- O = P·v: P fragments come straight from the S accumulator layout (two n-tiles = one k16 A fragment)
+            float oacc[4][4];
+#pragma unroll
+            for (int dt = 0; dt < 4; dt++)
+#pragma unroll
+                for (int e = 0; e < 4; e++) oacc[dt][e] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < 2; ks++) {
+                uint32_t ph[4], pl[4];
+                split2(sacc[2 * ks][0], sacc[2 * ks][1], ph[0], pl[0]);
+                split2(sacc[2 * ks][2], sacc[2 * ks][3], ph[1], pl[1]);
+                split2(sacc[2 * ks + 1][0], sacc[2 * ks + 1][1], ph[2], pl[2]);
+                split2(sacc[2 * ks + 1][2], sacc[2 * ks + 1][3], ph[3], pl[3]);
+#pragma unroll
+                for (int dp = 0; dp < 2; dp++) {
+                    uint32_t vh[4], vl[4];
+                    const uint32_t off = qa_off(ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, dp * 2 + (lane >> 4));
+                    ldsm_x4_trans(uVh + off, vh);
+                    ldsm_x4_trans(uVl + off, vl);
+#pragma unroll
+                    for (int j = 0; j < 2; j++) {
+                        mma16816(oacc[dp * 2 + j], ph, vh[2 * j], vh[2 * j + 1]);
+                        mma16816(oacc[dp * 2 + j], pl, vh[2 * j], vh[2 * j + 1]);
+                        mma16816(oacc[dp * 2 + j], ph, vl[2 * j], vl[2 * j + 1]);
+                    }
+                }
+            }
+            // ---- normalise, split, stage the warp's 16 output rows in its own q rows (only this warp reads them), store coalesced
+            uint32_t* sth = (uint32_t*)aQh;
+            uint32_t* stl = (uint32_t*)aQl;
+            __syncwarp();
+#pragma unroll
+            for (int hf = 0; hf < 2; hf++) {
+                const int row = mt * 16 + hf * 8 + gq;
+#pragma unroll
+                for (int dt = 0; dt < 4; dt++) {
+                    uint32_t hi, lo;
+                    split2(oacc[dt][2 * hf] * inv[hf], oacc[dt][2 * hf + 1] * inv[hf], hi, lo);
+                    const int w = row * 16 + ((dt ^ ((row >> 1) & 3)) << 2) + tq;
+                    sth[w] = hi;
+                    stl[w] = lo;
+                }
+            }
+            __syncwarp();
+            const size_t rb = ((size_t)tile * BM + pos * 32) * BN + h * 32;  // row 0 of this position, this head's columns
+#pragma unroll
+            for (int jj = 0; jj < 2; jj++) {
+                const int rr = mt * 16 + jj * 8 + (lane >> 2), cq = lane & 3;
+                const int w = rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2);
+                *(uint4*)(g.out_hi + rb + (size_t)rr * BN + cq * 8) = *(const uint4*)(sth + w);
+                *(uint4*)(g.out_lo + rb + (size_t)rr * BN + cq * 8) = *(const uint4*)(stl + w);
+            }
+            __syncwarp();
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == G_MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
     }
 }
 
@@ -1275,21 +718,15 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, con
 // operand is exact in bf16 (one-hot entries, and the normalised quality carried as two bf16 columns),
 // so two passes (A.W_hi + A.W_lo) reproduce the fp32 result.  Producers synthesise the swizzled A tile
 // straight from the [L',32] token/quality matrix (pad/zero rows of the reference batch as in k_stem).
-// Same skeleton as k_gemm_ws; one work item = 4 supported positions = 128 read tokens.
+// One work item = 4 supported positions = 128 read tokens.
 // ------------------------------------------------------------------------------------------------
 constexpr int STEM_STAGE_BYTES = (BM + 2 * BN) * 128;  // A (hi only) + W' hi/lo tiles of one k-block: 48 KB
 constexpr int STEM_MAXK = 64;                           // taps supported by the staging buffers
-constexpr int STEM_RP_LD = 132;                         // row stride (floats) of the read_pos copy: conflict-free 16-byte rows per lane
-// warps 0-7 epilogue (warp & 3 = TMEM lane quadrant = position of the item, warp >> 2 = column half), 8-11 producers, 12 MMA
-// 13-14 gather (token/quality neighbourhoods from the pileup matrix, one item ahead)
-constexpr int S_EPI = 256, S_PROD = 128, S_GATHER = 64, S_THREADS = 480, S_MMA_WARP = 12;
+constexpr int STEM_RP_LD = 132;                         // row stride (floats) of the read_pos copy
+// warps 0-7 consumers (two warpgroups), 8-11 producers (thread p synthesises row p of the A tile; one of them issues the
+// TMA of W'), 12-13 gather (token/quality neighbourhoods from the pileup matrix, one item ahead)
+constexpr int S_PROD = 128, S_GATHER = 64, S_THREADS = 448, S_GATHER_WARP = 12;
 
-#ifdef HB_FFN_TRACE
-__device__ unsigned long long hb_st_trace[4][2][32];  // [role: 0 MMA, 1 epilogue thread 0, 2 producer thread 0, 3 gather thread 0][item 10/11][event]
-#define TS_(role, k) do { if (blockIdx.x == 0 && (n_done == 10 || n_done == 11)) hb_st_trace[role][n_done - 10][k] = clock64(); } while (0)
-#else
-#define TS_(role, k) do { } while (0)
-#endif
 __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs g, const __grid_constant__ CUtensorMap tmWhi,
                                                          const __grid_constant__ CUtensorMap tmWlo) {
     extern __shared__ uint8_t smem_dyn[];
@@ -1297,11 +734,8 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
     uint8_t* tokbuf = smem + STAGES * STEM_STAGE_BYTES;          // [2][4 positions][STEM_MAXK taps][32] tokens
     uint8_t* qbuf = tokbuf + 2 * 4 * STEM_MAXK * 32;             // same shape, raw quality bytes
     float* s_rp = (float*)(qbuf + 2 * 4 * STEM_MAXK * 32);       // read_pos [32][STEM_RP_LD] (row 31 = zeros)
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], tfull_bar[2], tempty_bar[2], buf_full[2], buf_empty[2];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(16) float s_stage[8][32 * 16];  // per-warp transpose buffers (see warp_store_f32x16)
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], buf_full[2], buf_empty[2];
     __shared__ __align__(16) float s_bias[BN], s_lng[BN], s_lnb[BN];
-    __shared__ float s_red[2][2][BM];                    // [item parity][column half][row]: LayerNorm partial sums
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid < BN) {
@@ -1313,43 +747,30 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
         const int r = i >> 7, c = i & 127;
         s_rp[r * STEM_RP_LD + c] = r < R_COLS ? g.read_pos[i] : 0.f;
     }
-    if (warp == S_MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(2 * BN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], S_PROD + 1); mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], S_EPI);
-            mbar_init(&buf_full[a], S_GATHER); mbar_init(&buf_empty[a], S_PROD);
-        }
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], S_PROD + 1); mbar_init(&empty_bar[s], C_THREADS); }
+        for (int a = 0; a < 2; a++) { mbar_init(&buf_full[a], S_GATHER); mbar_init(&buf_empty[a], S_PROD); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
     const uint32_t n_items = (g.npos + 3) / 4;
     const uint32_t kbs = g.k_blocks;
     const int K = g.taps;
 
-    if (warp >= 8 && warp < 12) {
+    if (warp >= 8 && warp < S_GATHER_WARP) {
         // =============================== producers: thread p synthesises row p of the A tile ===============================
-        const int p = tid - S_EPI;
+        const int p = tid - C_THREADS;
         const int pos = p >> 5, rd = p & 31;
         uint32_t it_stage = 0, n_done = 0;
         for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
             const uint8_t* tb = tokbuf + (n_done & 1) * 4 * STEM_MAXK * 32;
             const uint8_t* qb = qbuf + (n_done & 1) * 4 * STEM_MAXK * 32;
-            if (p == 0) TS_(2, 0);
             mbar_wait(&buf_full[n_done & 1], (n_done >> 1) & 1);  // the gather warps have staged this item's neighbourhood
-            if (p == 0) TS_(2, 1);
             const uint8_t* trow = tb + pos * STEM_MAXK * 32 + rd;  // this row's token of tap j at trow[j * 32]
             const uint8_t* qrow = qb + pos * STEM_MAXK * 32 + rd;
             for (uint32_t kb = 0; kb < kbs; kb++, it_stage++) {
                 const uint32_t s = it_stage % STAGES, ph = (it_stage / STAGES) & 1;
                 mbar_wait(&empty_bar[s], ph ^ 1);
-                if (p == 0 && kb < 9) TS_(2, 2 + 2 * kb);
                 uint8_t* sA = smem + (size_t)s * STEM_STAGE_BYTES;
                 if (p == 0) {  // W' k-block (hi, lo) by TMA
                     mbar_arrive_expect_tx(&full_bar[s], 2 * BN * 128);
@@ -1358,8 +779,7 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                 }
                 // ---- A k-block: 4 taps x 16 features of this row, synthesised arithmetically: bf16 1.0 in the token's one-hot slot
                 //      (features 0..10; '.' has a slot, the pad token 11 and rows outside the reference batch are all zero) and the
-                //      normalised quality as (q_hi, q_lo) in features 11, 12.  (Round 1 looked both up in shared-memory tables: the 256-entry
-                //      quality table is indexed by data, i.e. 3-4-way bank conflicts on every look-up; ncu counted 43 M conflicts per launch.)
+                //      normalised quality as (q_hi, q_lo) in features 11, 12.
                 uint32_t tk[4], qq[4];
 #pragma unroll
                 for (int tl = 0; tl < 4; tl++) {
@@ -1388,16 +808,17 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                     *(uint4*)(sA + (uint32_t)p * 128u + (uint32_t)(((2 * tl) ^ (p & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
                     *(uint4*)(sA + (uint32_t)p * 128u + (uint32_t)(((2 * tl + 1) ^ (p & 7)) << 4)) = make_uint4(w[4], w[5], w[6], w[7]);
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                fence_async_smem();
                 mbar_arrive(&full_bar[s]);
-                if (p == 0 && kb < 9) TS_(2, 3 + 2 * kb);
             }
             mbar_arrive(&buf_empty[n_done & 1]);  // the staging buffer may be refilled
         }
-    } else if (warp > S_MMA_WARP) {
+        return;
+    }
+    if (warp >= S_GATHER_WARP) {
         // =============================== gather warps: stage the K x 32 token / quality neighbourhood of the 4 positions of
         // an item (double buffered, one item ahead of the synthesis, so the dependent global loads are off its critical path)
-        const int gt = tid - (S_MMA_WARP + 1) * 32;  // 0..63
+        const int gt = tid - S_GATHER_WARP * 32;  // 0..63
         uint32_t n_done = 0;
         for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
             uint8_t* tb = tokbuf + (n_done & 1) * 4 * STEM_MAXK * 32;
@@ -1410,9 +831,7 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                 m_row = b.fwd_row[g.n0 + item * 4 + lane];
                 m_L = b.w_L[w]; m_Lref = b.w_reflmax[w]; m_base = b.w_rowbase[w];
             }
-            if (gt == 0) TS_(3, 0);
             mbar_wait(&buf_empty[n_done & 1], ((n_done >> 1) & 1) ^ 1);
-            if (gt == 0) TS_(3, 1);
             for (int i0 = 0; i0 < 4 * K * 2; i0 += S_GATHER) {  // one 16-byte half row per iteration (warp-uniform trip count)
                 const int i = i0 + gt;
                 const int ps = min(i / (K * 2), 3), rem = i % (K * 2), j = rem >> 1, half = rem & 1;
@@ -1436,121 +855,57 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                 }
             }
             mbar_arrive(&buf_full[n_done & 1]);
-            if (gt == 0) TS_(3, 2);
         }
-    } else if (warp == S_MMA_WARP) {
-        // =============================== MMA issuer ===============================
-        if (lane == 0) {
-            uint32_t it_stage = 0, n_done = 0;
-            for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
-                const uint32_t acc = n_done & 1, aph = (n_done >> 1) & 1;
-                TS_(0, 0);
-                mbar_wait(&tempty_bar[acc], aph ^ 1);
-                TS_(0, 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (uint32_t kb = 0; kb < kbs; kb++, it_stage++) {
-                    const uint32_t s = it_stage % STAGES, ph = (it_stage / STAGES) & 1;
-                    mbar_wait(&full_bar[s], ph);
-                    if (kb < 9) TS_(0, 2 + kb);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t sb = smem_u32(smem + (size_t)s * STEM_STAGE_BYTES);
-                    const uint64_t dA = make_desc(sb);
-                    const uint64_t dBh = make_desc(sb + BM * 128), dBl = make_desc(sb + BM * 128 + BN * 128);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; k++) {
-                        const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                        mma_bf16(tmem_d, dA + adv, dBh + adv, (kb | (uint32_t)k) ? 1u : 0u);
-                        mma_bf16(tmem_d, dA + adv, dBl + adv, 1u);
-                    }
-                    umma_commit(&empty_bar[s]);
-                }
-                umma_commit(&tfull_bar[acc]);
-                TS_(0, 12);
-            }
-        }
-    } else if (warp < 8) {
-        // =============================== epilogue: relu(acc + bias) + read_pos (+ the first LayerNorm) ===============
-        const int wq = warp & 3, eh = warp >> 2, ch = eh * 64;
-        const float* rp = s_rp + lane * STEM_RP_LD + ch;   // row 31 (the pad token of every position) is zero
-        float* stg = s_stage[warp];
-        uint32_t n_done = 0;
-        for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x, n_done++) {
-            const uint32_t acc = n_done & 1, aph = (n_done >> 1) & 1;
-            if (tid == 0) TS_(1, 0);
-            mbar_wait(&tfull_bar[acc], aph);
-            if (tid == 0) TS_(1, 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // token row: position = item*4 + wq, read = lane
-            const uint32_t r = wq * 32 + lane;
-            const uint32_t taddr = tmem_base + acc * BN + ch + ((uint32_t)(wq * 32) << 16);
-            float* xblk = g.X + ((size_t)item * BM + wq * 32) * BN + ch;  // this warp's [32 rows][64 cols] block of X
-            float x[64];
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(taddr + (uint32_t)c0, v);
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 bv = *(const float4*)(s_bias + ch + c0 + j);
-                    const float4 pv = *(const float4*)(rp + c0 + j);
-                    x[c0 + j] = fmaxf(__uint_as_float(v[j]) + bv.x, 0.f) + pv.x; x[c0 + j + 1] = fmaxf(__uint_as_float(v[j + 1]) + bv.y, 0.f) + pv.y;
-                    x[c0 + j + 2] = fmaxf(__uint_as_float(v[j + 2]) + bv.z, 0.f) + pv.z; x[c0 + j + 3] = fmaxf(__uint_as_float(v[j + 3]) + bv.w, 0.f) + pv.w;
-                }
-                if (lane >= R_COLS) {  // the pad token of every position
-#pragma unroll
-                    for (int j = 0; j < 32; j++) x[c0 + j] = 0.f;
-                }
-                if (g.x_blocked) {  // tile-blocked residual stream: the row owner's 16-byte stores are coalesced as they are
-                    float* xt = g.X + (size_t)item * BM * BN + (size_t)((ch + c0) >> 2) * (BM * 4) + r * 4;
-#pragma unroll
-                    for (int q = 0; q < 8; q++)
-                        *(float4*)(xt + q * (BM * 4)) = make_float4(x[c0 + 4 * q], x[c0 + 4 * q + 1], x[c0 + 4 * q + 2], x[c0 + 4 * q + 3]);
-                } else {
-                    warp_store_f32x16(stg, lane, xblk + c0, BN, x + c0);
-                    warp_store_f32x16(stg, lane, xblk + c0 + 16, BN, x + c0 + 16);
-                }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&tempty_bar[acc]);
-            if (tid == 0) TS_(1, 2);
-            if (g.out_hi) {
-                // LayerNorm of the row (layer 0's ln1) -> split bf16: the operand of the first QKV projection.
-                // Partial sums are exchanged with the thread that owns the other 64 columns of the row.
-                float sum = 0.f;
-#pragma unroll
-                for (int j = 0; j < 64; j++) sum += x[j];
-                s_red[acc][eh][r] = sum;
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float mean = (s_red[acc][0][r] + s_red[acc][1][r]) * (1.f / BN);
-                float var = 0.f;
-#pragma unroll
-                for (int j = 0; j < 64; j++) { const float d = x[j] - mean; var = fmaf(d, d, var); }
-                asm volatile("bar.sync 2, 256;" ::: "memory");  // both halves have read the sums
-                s_red[acc][eh][r] = var;
-                asm volatile("bar.sync 2, 256;" ::: "memory");
-                const float rstd = rsqrtf((s_red[acc][0][r] + s_red[acc][1][r]) * (1.f / BN) + 1e-5f);
-                if (tid == 0) TS_(1, 3);
-                __nv_bfloat16* hblk = g.out_hi + ((size_t)item * BM + wq * 32) * BN + ch;
-                __nv_bfloat16* lblk = g.out_lo + ((size_t)item * BM + wq * 32) * BN + ch;
-#pragma unroll
-                for (int j = 0; j < 64; j += 16) {
-                    uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int e = 0; e < 16; e += 2)
-                        split2((x[j + e] - mean) * rstd * s_lng[ch + j + e] + s_lnb[ch + j + e],
-                               (x[j + e + 1] - mean) * rstd * s_lng[ch + j + e + 1] + s_lnb[ch + j + e + 1], hi[e >> 1], lo[e >> 1]);
-                    warp_store_bf16x16((uint32_t*)stg, lane, hblk + j, BN, hi);
-                    warp_store_bf16x16((uint32_t*)stg, lane, lblk + j, BN, lo);
-                }
-                if (tid == 0) TS_(1, 4);
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == S_MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * BN));
+    // =============================== consumers: wgmma, then relu(acc + bias) + read_pos (+ the first LayerNorm) ==========
+    const int wg = warp >> 2;
+    const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), fc = (lane & 3) * 2;
+    const int rd0 = fr & 31, rd1 = (fr + 8) & 31;  // read token (row of the position) of the two fragment rows
+    uint32_t it_stage = 0;
+    float acc[64];
+    for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < kbs; kb++, it_stage++) {
+            const uint32_t s = it_stage % STAGES, ph = (it_stage / STAGES) & 1;
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sb = smem_u32(smem + (size_t)s * STEM_STAGE_BYTES);
+            const uint64_t dA = make_desc(sb + wg * 64 * 128), dBh = make_desc(sb + BM * 128), dBl = make_desc(sb + BM * 128 + BN * 128);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; k++) {
+                const uint64_t adv = (uint64_t)(k * 2);
+                wgmma_n128(acc, dA + adv, dBh + adv, (kb | (uint32_t)k) ? 1u : 0u);
+                wgmma_n128(acc, dA + adv, dBl + adv, 1u);
+            }
+            wg_commit();
+            if (kb > 0) {
+                wg_wait<1>();
+                mbar_arrive(&empty_bar[prev]);
+            }
+            prev = s;
+        }
+        wg_wait<0>();
+        acc_fence(acc);
+        mbar_arrive(&empty_bar[prev]);
+        const size_t row0 = (size_t)item * BM + fr;
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const int c = 8 * j + fc;
+            const float* rp0 = s_rp + rd0 * STEM_RP_LD + c;
+            const float* rp1 = s_rp + rd1 * STEM_RP_LD + c;
+            acc[4 * j] = fmaxf(acc[4 * j] + s_bias[c], 0.f) + rp0[0];
+            acc[4 * j + 1] = fmaxf(acc[4 * j + 1] + s_bias[c + 1], 0.f) + rp0[1];
+            acc[4 * j + 2] = fmaxf(acc[4 * j + 2] + s_bias[c], 0.f) + rp1[0];
+            acc[4 * j + 3] = fmaxf(acc[4 * j + 3] + s_bias[c + 1], 0.f) + rp1[1];
+            if (rd0 >= R_COLS) { acc[4 * j] = 0.f; acc[4 * j + 1] = 0.f; }  // the pad token of every position
+            if (rd1 >= R_COLS) { acc[4 * j + 2] = 0.f; acc[4 * j + 3] = 0.f; }
+        }
+        frag_store_f32(acc, g.X, BN, row0, 0, fc);
+        if (g.out_hi) {  // LayerNorm of the row (layer 0's ln1) -> split bf16: the operand of the first QKV projection
+            frag_layernorm(acc, s_lng, s_lnb, fc);
+            frag_store_split(acc, g.out_hi, g.out_lo, BN, row0, 0, fc);
+        }
     }
 }
 
@@ -1630,33 +985,17 @@ cudaError_t ffn_tc(const FfnArgs& a, int num_sms, cudaStream_t st) {
         configured = true;
     }
     if (a.m_tiles == 0) return cudaSuccess;
-    CUtensorMap tHh, tHl, t1h, t1l, t2h, t2l, toh, tol, tOh, tOl;
+    CUtensorMap tHh, tHl, t1h, t1l, t2h, t2l, toh, tol;
     const uint64_t T = (uint64_t)a.m_tiles * BM;
     if (!make_tmap(&tHh, a.Hhi, T, BN, BN) || !make_tmap(&tHl, a.Hlo, T, BN, BN) || !make_tmap(&t1h, a.W1hi, a.F, BN, BN) ||
         !make_tmap(&t1l, a.W1lo, a.F, BN, BN) || !make_tmap(&t2h, a.W2hi, BN, a.F, a.F) || !make_tmap(&t2l, a.W2lo, BN, a.F, a.F))
         return cudaErrorInvalidValue;
-    if (!make_tmap(&tOh, a.out_hi, T, BN, BN) || !make_tmap(&tOl, a.out_lo, T, BN, BN)) return cudaErrorInvalidValue;
     const unsigned grid = (unsigned)std::min<uint32_t>(a.m_tiles, (uint32_t)num_sms);
     if (a.Wohi) {
         if (!make_tmap(&toh, a.Wohi, BN, BN, BN) || !make_tmap(&tol, a.Wolo, BN, BN, BN)) return cudaErrorInvalidValue;
-        k_ffn_ws<true><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, toh, tol, tOh, tOl);
-#ifdef HB_FFN_TRACE
-        static int calls = 0;
-        if (++calls == 25 && a.m_tiles > 148 * 12) {
-            cudaStreamSynchronize(st);
-            static unsigned long long h[3][2][64];
-            cudaMemcpyFromSymbol(h, hb_ffn_trace, sizeof(h));
-            const unsigned long long t0 = h[0][0][0];
-            for (int r = 0; r < 3; r++)
-                for (int t = 0; t < 2; t++) {
-                    fprintf(stderr, "FFNTRACE role %d tile %d:", r, t);
-                    for (int k = 0; k < 64; k++) fprintf(stderr, " %lld", h[r][t][k] ? (long long)(h[r][t][k] - t0) : -1LL);
-                    fprintf(stderr, "\n");
-                }
-        }
-#endif
+        k_ffn_ws<true><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, toh, tol);
     } else {
-        k_ffn_ws<false><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, t1h, t1l, tOh, tOl);
+        k_ffn_ws<false><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, t1h, t1l);
     }
     return cudaGetLastError();
 }
@@ -1674,27 +1013,12 @@ cudaError_t stem_tc(const BatchView& b, const StemArgs& a, int num_sms, cudaStre
     CUtensorMap tWh, tWl;
     if (!make_tmap(&tWh, a.Whi, BN, a.Kp, a.Kp) || !make_tmap(&tWl, a.Wlo, BN, a.Kp, a.Kp)) return cudaErrorInvalidValue;
     k_stem_tc<<<(unsigned)std::min<uint32_t>(items, (uint32_t)num_sms), S_THREADS, smem, st>>>(b, a, tWh, tWl);
-#ifdef HB_FFN_TRACE
-    static int calls = 0;
-    if (++calls == 13 && items > 148 * 12) {
-        cudaStreamSynchronize(st);
-        static unsigned long long h[4][2][32];
-        cudaMemcpyFromSymbol(h, hb_st_trace, sizeof(h));
-        const unsigned long long t0 = h[0][0][0];
-        for (int r = 0; r < 4; r++)
-            for (int t = 0; t < 2; t++) {
-                fprintf(stderr, "STTRACE role %d item %d:", r, t);
-                for (int k = 0; k < 22; k++) fprintf(stderr, " %lld", h[r][t][k] ? (long long)(h[r][t][k] - t0) : -1LL);
-                fprintf(stderr, "\n");
-            }
-    }
-#endif
     return cudaGetLastError();
 }
 
 cudaError_t qkv_attn_tc(const QkvAttnArgs& a, int num_sms, cudaStream_t st) {
     static bool configured = false;
-    const size_t smem = (size_t)FFN_A_BYTES + (size_t)QA_STAGES * QA_RING_BYTES + (size_t)8 * QA_WARP_BYTES + 1024;
+    const size_t smem = (size_t)FFN_A_BYTES + (size_t)QA_STAGES * QA_RING_BYTES + (size_t)4 * QA_POS_BYTES + 1024;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(k_qkv_attn_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -1707,21 +1031,6 @@ cudaError_t qkv_attn_tc(const QkvAttnArgs& a, int num_sms, cudaStream_t st) {
         !make_tmap(&tWl, a.Wlo, 4 * QA_HROWS, BN, BN, QA_HROWS))
         return cudaErrorInvalidValue;
     k_qkv_attn_ws<<<(unsigned)std::min<uint32_t>(a.m_tiles, (uint32_t)num_sms), G_THREADS, smem, st>>>(a, tHh, tHl, tWh, tWl);
-#ifdef HB_FFN_TRACE
-    static int calls = 0;
-    if (++calls == 25 && a.m_tiles > 148 * 12) {
-        cudaStreamSynchronize(st);
-        static unsigned long long h[3][2][64];
-        cudaMemcpyFromSymbol(h, hb_qa_trace, sizeof(h));
-        const unsigned long long t0 = h[0][0][0];
-        for (int r = 0; r < 3; r++)
-            for (int t = 0; t < 2; t++) {
-                fprintf(stderr, "QATRACE role %d tile %d:", r, t);
-                for (int k = 0; k < 24; k++) fprintf(stderr, " %lld", h[r][t][k] ? (long long)(h[r][t][k] - t0) : -1LL);
-                fprintf(stderr, "\n");
-            }
-    }
-#endif
     return cudaGetLastError();
 }
 

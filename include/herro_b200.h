@@ -1,4 +1,4 @@
-/* herro_b200.h — C ABI of the B200-native HERRO hot path (features -> inference -> consensus).
+/* herro_b200.h — C ABI of the H100-native HERRO hot path (features -> inference -> consensus).
  *
  * The reference (lbcb-sci/herro @ 9cd0296) has no FFI layer: the three stages are Rust
  * worker threads joined by crossbeam channels.  This header is what a `mod ffi` in the Rust
@@ -216,7 +216,7 @@ int hb_dump_features(hb_ctx* ctx, uint32_t rid, const char* out_dir, const char*
 int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms);
 
 /* ---- diagnostics ------------------------------------------------------------------------- */
-/* Runs the tcgen05 (bf16x3) contraction kernel and the fp32 SIMT one on the same random
+/* Runs the wgmma (bf16x3) contraction kernel and the fp32 SIMT one on the same random
  * [M,K]x[N,K]^T problem (M % 128 == 0, N % 128 == 0, K % 64 == 0; lda = K + lda_extra; act: 0 none,
  * 1 ReLU, 2 ReLU with split-bf16 output; res: add a residual) and reports the largest absolute
  * difference, the largest |reference| and both kernel times. */

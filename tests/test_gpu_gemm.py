@@ -1,4 +1,4 @@
-"""tcgen05 (bf16x3 split) contraction kernel vs the fp32 SIMT kernel on random data."""
+"""wgmma (bf16x3 split) contraction kernel vs the fp32 SIMT kernel on random data."""
 import pytest
 
 from herro_b200 import api

@@ -1,15 +1,15 @@
 #!/usr/bin/env python
-"""profiles/<round>_sass_summary.txt: per-kernel SASS opcode evidence of the built library (cuobjdump -sass), so that the
-tcgen05 / TMA / TMEM claims can be checked without disassembling an untracked .so.
-    python tools/sass_summary.py herro_b200/libherro_b200.so profiles/r02_sass_summary.txt
-Mnemonics (B200_PROFILING.md): UTCHMMA/UTCQMMA = tcgen05.mma, UTMALDG = cp.async.bulk.tensor (TMA), LDTM/STTM = tcgen05.ld/st,
-UTCBAR = tcgen05.commit, HMMA = mma.sync, SYNCS = mbarrier."""
+"""Per-kernel SASS opcode counts of the built library (cuobjdump -sass), so that the wgmma / TMA claims can be checked
+without disassembling the .so by hand.
+    python tools/sass_summary.py herro_b200/libherro_b200.so OUT.txt
+Mnemonics on sm_90a: HGMMA = wgmma.mma_async, UTMALDG = cp.async.bulk.tensor (TMA), HMMA = mma.sync, LDSM = ldmatrix,
+SYNCS = mbarrier."""
 import collections
 import re
 import subprocess
 import sys
 
-KEY = ["UTCHMMA", "UTCQMMA", "UTCOMMA", "UTMALDG", "UTMASTG", "LDTM", "STTM", "UTCBAR", "UTCATOM", "SYNCS", "HMMA", "LDSM", "LDG", "STG", "LDS",
+KEY = ["HGMMA", "WARPSYNC", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "LDSM", "LDG", "STG", "LDS",
        "STS", "ATOMS", "ATOMG", "PRMT", "POPC", "SHFL", "BAR", "LOP3", "IMAD", "FFMA", "MUFU"]
 
 
