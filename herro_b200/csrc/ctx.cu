@@ -60,37 +60,18 @@ struct AllocScope {
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
-    cudaStream_t st = nullptr;  // lane buffers: grown in stream order from the device's memory pool, because
+    cudaStream_t st = nullptr;  // lane regions: grown in stream order from the device's memory pool, because
                                 // cudaMalloc/cudaFree synchronise the whole device and would stall the other lanes
-    cudaError_t ensure(size_t bytes, bool keep = false) {
+    // Grow to hold `bytes`: with 1.5x headroom, or exactly (pre-sizing an idle lane from another lane's sizes).  `keep` copies
+    // the contents over (a pre-sized lane's last launch stays replayable / inspectable through the debug taps).
+    cudaError_t grow(size_t bytes, bool headroom = true, bool keep = false) {
         if (bytes <= cap) return cudaSuccess;
-        size_t ncap = bytes + bytes / 2 + 256;
+        const size_t ncap = headroom ? bytes + bytes / 2 + 256 : bytes;
         AllocScope as_(st ? "device(stream-ordered)" : "device", ncap);
-        void* np = nullptr;
-        if (st) {
-            cudaError_t e = cudaMallocAsync(&np, ncap, st);
-            if (e != cudaSuccess) return e;
-            if (keep && p && cap) cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, st);
-            if (p) cudaFreeAsync(p, st);
-        } else {
-            cudaError_t e = cudaMalloc(&np, ncap);
-            if (e != cudaSuccess) return e;
-            if (keep && p && cap) cudaMemcpy(np, p, cap, cudaMemcpyDeviceToDevice);
-            if (p) cudaFree(p);
-        }
-        p = np;
-        cap = ncap;
-        return cudaSuccess;
-    }
-    // grow to exactly `ncap` bytes without headroom (pre-sizing an idle lane from another lane's sizes); contents are kept
-    // (the lane's last launch stays replayable / inspectable through the debug taps)
-    cudaError_t reserve_exact(size_t ncap) {
-        if (ncap <= cap) return cudaSuccess;
-        AllocScope as_(st ? "device(stream-ordered, presize)" : "device(presize)", ncap);
         void* np = nullptr;
         cudaError_t e = st ? cudaMallocAsync(&np, ncap, st) : cudaMalloc(&np, ncap);
         if (e != cudaSuccess) return e;
-        if (p && cap) { if (st) cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, st); else cudaMemcpy(np, p, cap, cudaMemcpyDeviceToDevice); }
+        if (keep && p) { if (st) cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, st); else cudaMemcpy(np, p, cap, cudaMemcpyDeviceToDevice); }
         if (p) { if (st) cudaFreeAsync(p, st); else cudaFree(p); }
         p = np;
         cap = ncap;
@@ -103,20 +84,11 @@ struct DevBuf {
 struct PinBuf {
     void* p = nullptr;
     size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
+    // grow to hold `bytes`, with 1.5x headroom or exactly; the contents are not kept
+    cudaError_t grow(size_t bytes, bool headroom = true) {
         if (bytes <= cap) return cudaSuccess;
-        AllocScope as_("pinned(lane)", bytes + bytes / 2 + 256);
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        size_t ncap = bytes + bytes / 2 + 256;
-        cudaError_t e = cudaMallocHost(&p, ncap);
-        if (e == cudaSuccess) cap = ncap;
-        return e;
-    }
-    cudaError_t reserve_exact(size_t ncap) {
-        if (ncap <= cap) return cudaSuccess;
-        AllocScope as_("pinned(lane, presize)", ncap);
+        const size_t ncap = headroom ? bytes + bytes / 2 + 256 : bytes;
+        AllocScope as_("pinned(lane)", ncap);
         if (p) cudaFreeHost(p);
         p = nullptr;
         cap = 0;
@@ -198,6 +170,11 @@ struct Result {
     std::string msg;  // why status != HB_OK
 };
 
+struct FwdBufs {  // the forward region's arrays besides the work list, which is part of BatchView
+    float *logits, *info;
+    uint8_t* ws;
+};
+
 struct LastLaunch {  // host copies of per-window metadata of the most recent launch (debug taps / replay)
     bool valid = false;
     std::vector<DevWin> win;
@@ -206,7 +183,11 @@ struct LastLaunch {  // host copies of per-window metadata of the most recent la
     std::vector<uint32_t> ow_qid;  // KEEP_DEBUG: query read of every overlap-window (feature dump)
     std::unordered_map<uint64_t, uint32_t> index;  // (rid << 32 | wid) -> window
     uint64_t n_sup = 0, total_rows = 0;
+    // the counts the lane's scratch was carved from, besides those in `view` (a pre-sized lane carves the view again)
+    size_t cig_bytes = 0;
+    uint64_t op_slots = 0, raw_slots = 0;
     BatchView view;
+    FwdBufs fwd;
 };
 
 }  // namespace
@@ -240,42 +221,26 @@ struct hb_ctx {
         cudaStream_t stream = nullptr;
         cudaEvent_t ev[8]{};
         KTimer kt;
-        PinBuf pin_small, pin_out;
-        DevBuf d_tgt, d_win, d_ovl, d_ow, d_cig;
-        DevBuf d_op_kl, d_op_t, d_op_q, d_ow_nops, d_ow_flags, d_ow_acc, d_ow_tend, d_col_ow, d_w_n1, d_w_S;
-        DevBuf d_ovl_n, d_ovl_tot, d_ovl_score, d_sel_ow, d_w_nsel, d_rowmap, d_w_L, d_w_rowbase, d_w_nsup, d_w_reflmax;
-        DevBuf d_mat_b, d_mat_q, d_row_emit, d_sup_row, d_sup_pk, d_w_supbase, d_fwd_win, d_fwd_row;
-        DevBuf d_w_outlen, d_w_outoff, d_out, d_tgt_err, d_counters, d_ws, d_logits, d_info, d_big_key, d_big_cand, d_big_score;
-        DevBuf d_raw_kl, d_raw_t, d_raw_q, d_aln_nops, d_aln_flags, d_ow_opoff;  // device windowing (windowing_dev.cu)
-        DevBuf d_rank_ow;
+        // device scratch, one region per moment its size becomes known: the batch (carve_batch), the row arena (carve_rows)
+        // and the supported positions (carve_fwd)
+        DevBuf d_batch, d_rows, d_fwd;
+        PinBuf pin_small, pin_out;  // readback of the counters and per-window metadata (carve_readback), of the emitted bytes
         uint64_t rows_cap = 0;
         uint64_t seen_sizes = 0;  // version of hb_ctx::lane_sizes this lane has been pre-sized to
         LastLaunch last;
         std::thread worker;
-        static constexpr int N_DEV = 51;
-        void all_bufs(DevBuf* (&out)[N_DEV]) {
-            DevBuf* bufs[N_DEV] = {&d_tgt, &d_win, &d_ovl, &d_ow, &d_cig, &d_op_kl, &d_op_t, &d_op_q, &d_ow_nops, &d_ow_flags, &d_ow_acc,
-                                   &d_ow_tend, &d_col_ow, &d_w_n1, &d_w_S, &d_ovl_n, &d_ovl_tot, &d_ovl_score, &d_sel_ow, &d_w_nsel,
-                                   &d_rowmap, &d_w_L, &d_w_rowbase, &d_w_nsup, &d_w_reflmax, &d_mat_b, &d_mat_q, &d_row_emit, &d_sup_row,
-                                   &d_sup_pk, &d_w_supbase, &d_fwd_win, &d_fwd_row, &d_w_outlen, &d_w_outoff, &d_out, &d_tgt_err,
-                                   &d_counters, &d_ws, &d_logits, &d_info, &d_big_key, &d_big_cand, &d_big_score,
-                                   &d_raw_kl, &d_raw_t, &d_raw_q, &d_aln_nops, &d_aln_flags, &d_ow_opoff, &d_rank_ow};
-            for (int i = 0; i < N_DEV; i++) out[i] = bufs[i];
-        }
-        void bind_stream() { DevBuf* bufs[N_DEV]; all_bufs(bufs); for (DevBuf* b : bufs) b->st = stream; }
         void release() {
-            DevBuf* bufs[N_DEV]; all_bufs(bufs);
-            for (DevBuf* b : bufs) b->release();
+            d_batch.release(); d_rows.release(); d_fwd.release();
             pin_small.release(); pin_out.release();
             for (auto& e : ev) if (e) cudaEventDestroy(e);
             kt.destroy();
             if (stream) cudaStreamDestroy(stream);
         }
     };
-    // Largest buffer capacities any lane has needed so far.  A lane that has not run yet (or ran smaller batches) grows its
-    // buffers to these while it is idle, so that its first real batch allocates nothing (r01: 26 allocations / 226 ms inside the
-    // timed region at 8 GPUs, when host contention made the third lane start its first batch there).
-    struct LaneSizes { size_t dev[Lane::N_DEV] = {0}; size_t pin_small = 0, pin_out = 0; uint64_t rows_cap = 0; };
+    // Largest region capacities (and row arena) any lane has needed so far.  A lane that has not run yet (or ran smaller batches)
+    // grows its regions to these while it is idle, so that its first real batch allocates nothing (r01: 26 allocations / 226 ms
+    // inside the timed region at 8 GPUs, when host contention made the third lane start its first batch there).
+    struct LaneSizes { size_t batch = 0, rows = 0, fwd = 0, pin_small = 0, pin_out = 0; uint64_t rows_cap = 0; };
     LaneSizes lane_sizes;
     uint64_t lane_sizes_version = 0;
     static constexpr int MAX_LANES = 4;
@@ -564,138 +529,135 @@ int load_weights(hb_ctx* ctx, const char* path) {
 template <class T>
 size_t vbytes(const PinVec<T>& v) { return v.size() * sizeof(T); }
 
-int ensure_batch_buffers(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt) {
-    const size_t nt = hbt.tgt.size(), nw = hbt.win.size(), no = hbt.ovl.size(), now_ = hbt.ow.size();
-    const uint32_t W = ctx->opt.window_size;
-    CK(L->d_tgt.ensure(nt * sizeof(DevTarget)));
-    CK(L->d_win.ensure(nw * sizeof(DevWin)));
-    CK(L->d_ovl.ensure(std::max<size_t>(no, 1) * sizeof(DevOverlap)));
-    CK(L->d_ow.ensure(std::max<size_t>(now_, 1) * sizeof(DevOW)));
-    CK(L->d_cig.ensure(std::max<size_t>(hbt.cig.size(), 16)));
-    const size_t opc = std::max<uint64_t>(hbt.op_cap + hbt.dev_op_cap, 1);
-    if (opc >= 0xffffffffull) return fail(ctx, HB_ERR_CAPACITY, "batch too large: more than 2^32 CIGAR ops (lower launch_targets)");
-    const size_t rawc = std::max<uint64_t>(hbt.raw_cap, 1);
-    CK(L->d_raw_kl.ensure(rawc * 4));
-    CK(L->d_raw_t.ensure(rawc * 4));
-    CK(L->d_raw_q.ensure(rawc * 4));
-    CK(L->d_op_kl.ensure(opc * 4));
-    CK(L->d_op_t.ensure(opc * 4));
-    CK(L->d_op_q.ensure(opc * 4));
-    const size_t ow1 = std::max<size_t>(now_, 1);
-    CK(L->d_ow_nops.ensure(ow1 * 4));
-    CK(L->d_ow_flags.ensure(ow1 * 4));
-    CK(L->d_ow_acc.ensure(ow1 * 4));
-    CK(L->d_ow_tend.ensure(ow1 * 4));
-    CK(L->d_col_ow.ensure(ow1 * 4));
-    CK(L->d_big_key.ensure(ow1 * 4));
-    CK(L->d_big_cand.ensure(ow1 * 4));
-    CK(L->d_big_score.ensure(ow1 * 8));
-    CK(L->d_ow_opoff.ensure(ow1 * 8));
-    CK(L->d_rank_ow.ensure(ow1 * 4));
-    CK(L->d_w_n1.ensure(nw * 4));
-    CK(L->d_w_S.ensure(nw * 4));
-    const size_t no1 = std::max<size_t>(no, 1);
-    CK(L->d_ovl_n.ensure(no1 * 4));
-    CK(L->d_ovl_tot.ensure(no1 * 4));
-    CK(L->d_ovl_score.ensure(no1 * 8));
-    CK(L->d_aln_nops.ensure(no1 * 4));
-    CK(L->d_aln_flags.ensure(no1 * 4));
-    CK(L->d_sel_ow.ensure(nw * TOP_K * 4));
-    CK(L->d_w_nsel.ensure(nw * 4));
-    CK(L->d_rowmap.ensure(nw * (size_t)(W + 1) * 4));
-    CK(L->d_w_L.ensure(nw * 4));
-    CK(L->d_w_rowbase.ensure(nw * 8));
-    CK(L->d_w_nsup.ensure(nw * 4));
-    CK(L->d_w_reflmax.ensure(nw * 4));
-    CK(L->d_w_supbase.ensure(nw * 8));
-    CK(L->d_w_outlen.ensure(nw * 4));
-    CK(L->d_w_outoff.ensure(nw * 8));
-    CK(L->d_tgt_err.ensure(nt * 4));
-    CK(L->d_counters.ensure(CNT_N * 4));
-    return HB_OK;
+// A lane's scratch regions are carved the way forward.cu carves the forward workspace: every array starts 256-byte aligned and
+// the layout depends only on the counts, so a dry run (base == nullptr) gives a region's size, and carving the same counts
+// again after the region moved with its contents gives the same offsets.
+struct Carve {
+    uint8_t* base;
+    size_t bytes = 0;
+    template <class T> void operator()(T*& p, size_t n) { p = (T*)(base + bytes); bytes += al256(n * sizeof(T)); }
+};
+
+// Batch region, sized from the HostBatch when a launch starts (the view's n_tgt / n_win / n_ovl / n_ow and W, and the CIGAR
+// bytes and op slots): inputs, raw and tokenised ops, everything per overlap-window, overlap, window and target, counters.
+size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t raw_slots, uint8_t* base) {
+    const size_t nt = b.n_tgt, nw = b.n_win, no1 = std::max<size_t>(b.n_ovl, 1), ow1 = std::max<size_t>(b.n_ow, 1);
+    const size_t ops = std::max<uint64_t>(op_slots, 1), raw = std::max<uint64_t>(raw_slots, 1);
+    Carve c{base};
+    c(b.tgt, nt);
+    c(b.win, nw);
+    c(b.ovl, no1);
+    c(b.ow_mut, ow1);
+    b.ow = b.ow_mut;
+    c(b.cig, std::max<size_t>(cig_bytes, 16));
+    c(b.raw_kl, raw);
+    c(b.raw_t, raw);
+    c(b.raw_q, raw);
+    c(b.op_kl, ops);
+    c(b.op_t, ops);
+    c(b.op_q, ops);
+    c(b.ow_nops, ow1);
+    c(b.ow_flags, ow1);
+    c(b.ow_acc, ow1);
+    c(b.ow_tend, ow1);
+    c(b.col_ow, ow1);
+    c(b.big_key, ow1);
+    c(b.big_cand, ow1);
+    c(b.big_score, ow1);
+    c(b.ow_opoff, ow1);
+    c(b.rank_ow, ow1);
+    c(b.ovl_n, no1);
+    c(b.ovl_tot, no1);
+    c(b.ovl_score, no1);
+    c(b.aln_nops, no1);
+    c(b.aln_flags, no1);
+    c(b.w_n1, nw);
+    c(b.w_S, nw);
+    c(b.sel_ow, nw * TOP_K);
+    c(b.w_nsel, nw);
+    c(b.rowmap, nw * (size_t)(b.W + 1));
+    c(b.w_L, nw);
+    c(b.w_rowbase, nw);
+    c(b.w_nsup, nw);
+    c(b.w_reflmax, nw);
+    c(b.w_supbase, nw);
+    c(b.w_outlen, nw);
+    c(b.w_outoff, nw);
+    c(b.tgt_err, nt);
+    c(b.counters, CNT_N);
+    return c.bytes;
 }
 
-int ensure_row_buffers(hb_ctx* ctx, hb_ctx::Lane* L, uint64_t rows) {
-    if (rows <= L->rows_cap) return HB_OK;
-    CK(L->d_mat_b.ensure(rows * ROW_BYTES));
-    CK(L->d_mat_q.ensure(rows * ROW_BYTES));
-    CK(L->d_row_emit.ensure(rows));
-    CK(L->d_sup_row.ensure(rows * 4));
-    CK(L->d_sup_pk.ensure(rows * 4));
-    CK(L->d_out.ensure(rows));
-    L->rows_cap = rows;
-    return HB_OK;
+// Row region, sized from the row arena (the view's rows_cap)
+size_t carve_rows(BatchView& b, uint8_t* base) {
+    const size_t rows = b.rows_cap;
+    Carve c{base};
+    c(b.mat_bases, rows * ROW_BYTES);
+    c(b.mat_quals, rows * ROW_BYTES);
+    c(b.row_emit, rows);
+    c(b.sup_row, rows);
+    c(b.sup_pk, rows);
+    c(b.out_bytes, rows);
+    return c.bytes;
 }
 
-// the pointer fields of a view: the lane's buffers as they are now
-void set_view_ptrs(hb_ctx* ctx, hb_ctx::Lane* L, BatchView& b) {
+// Forward region, sized from the supported positions once the first wait has counted them: the work list, the logits and
+// the workspace of one forward pass
+size_t carve_fwd(const hb_ctx* ctx, BatchView& b, FwdBufs& f, uint64_t n_sup, uint8_t* base) {
+    const size_t n = std::max<uint64_t>(n_sup, 1);
+    Carve c{base};
+    c(b.fwd_win, n);
+    c(b.fwd_row, n);
+    c(f.logits, n * 5);
+    c(f.info, n);
+    c(f.ws, fwd_workspace_bytes(ctx->wt, (uint32_t)std::min<uint64_t>(ctx->chunk_pos, n)));
+    return c.bytes;
+}
+
+// Pinned readback of a launch: counters, then per window and per target what the per-read reassembly needs
+struct Readback {
+    uint32_t *cnt, *outlen, *nsel, *L, *nsup, *terr, *sel;
+};
+size_t carve_readback(Readback& h, size_t nt, size_t nw, uint8_t* base) {
+    Carve c{base};
+    c(h.cnt, CNT_N);
+    c(h.outlen, nw);
+    c(h.nsel, nw);
+    c(h.L, nw);
+    c(h.nsup, nw);
+    c(h.terr, nt);
+    c(h.sel, nw * TOP_K);
+    return c.bytes;
+}
+
+// The counts of a launch and the context's read store; the scratch pointers are carved from the lane's regions.
+BatchView make_view(hb_ctx* ctx, const HostBatch& hbt) {
+    BatchView b{};
     b.rs = ctx->rs;
-    b.tgt = L->d_tgt.as<DevTarget>();
-    b.win = L->d_win.as<DevWin>();
-    b.ovl = L->d_ovl.as<DevOverlap>();
-    b.ow = L->d_ow.as<DevOW>();
-    b.ow_mut = L->d_ow.as<DevOW>();
-    b.raw_kl = L->d_raw_kl.as<uint32_t>();
-    b.raw_t = L->d_raw_t.as<uint32_t>();
-    b.raw_q = L->d_raw_q.as<uint32_t>();
-    b.aln_nops = L->d_aln_nops.as<uint32_t>();
-    b.aln_flags = L->d_aln_flags.as<uint32_t>();
-    b.ow_opoff = L->d_ow_opoff.as<uint64_t>();
-    b.cig = L->d_cig.as<uint8_t>();
-    b.op_kl = L->d_op_kl.as<uint32_t>();
-    b.op_t = L->d_op_t.as<uint32_t>();
-    b.op_q = L->d_op_q.as<uint32_t>();
-    b.ow_nops = L->d_ow_nops.as<uint32_t>();
-    b.ow_flags = L->d_ow_flags.as<uint32_t>();
-    b.ow_acc = L->d_ow_acc.as<float>();
-    b.ow_tend = L->d_ow_tend.as<uint32_t>();
-    b.col_ow = L->d_col_ow.as<uint32_t>();
-    b.big_key = L->d_big_key.as<float>();
-    b.big_cand = L->d_big_cand.as<uint32_t>();
-    b.big_score = L->d_big_score.as<double>();
-    b.w_n1 = L->d_w_n1.as<uint32_t>();
-    b.w_S = L->d_w_S.as<uint32_t>();
-    b.ovl_n = L->d_ovl_n.as<uint32_t>();
-    b.ovl_tot = L->d_ovl_tot.as<uint32_t>();
-    b.ovl_score = L->d_ovl_score.as<double>();
     b.ln_table = ctx->d_ln.as<double>();
     b.ln_table_n = ctx->ln_n;
-    b.rank_ow = L->d_rank_ow.as<uint32_t>();
-    b.sel_ow = L->d_sel_ow.as<uint32_t>();
-    b.w_nsel = L->d_w_nsel.as<uint32_t>();
-    b.rowmap = L->d_rowmap.as<uint32_t>();
-    b.w_L = L->d_w_L.as<uint32_t>();
-    b.w_rowbase = L->d_w_rowbase.as<uint64_t>();
-    b.w_nsup = L->d_w_nsup.as<uint32_t>();
-    b.w_reflmax = L->d_w_reflmax.as<uint32_t>();
-    b.mat_bases = L->d_mat_b.as<uint8_t>();
-    b.mat_quals = L->d_mat_q.as<uint8_t>();
-    b.row_emit = L->d_row_emit.as<uint8_t>();
-    b.sup_row = L->d_sup_row.as<uint32_t>();
-    b.sup_pk = L->d_sup_pk.as<uint32_t>();
-    b.w_supbase = L->d_w_supbase.as<uint64_t>();
-    b.fwd_win = L->d_fwd_win.as<uint32_t>();
-    b.fwd_row = L->d_fwd_row.as<uint32_t>();
-    b.w_outlen = L->d_w_outlen.as<uint32_t>();
-    b.w_outoff = L->d_w_outoff.as<uint64_t>();
-    b.out_bytes = L->d_out.as<uint8_t>();
-    b.tgt_err = L->d_tgt_err.as<uint32_t>();
-    b.counters = L->d_counters.as<uint32_t>();
-}
-
-BatchView make_view(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt) {
-    BatchView b{};
     b.W = ctx->opt.window_size;
     b.n_tgt = (uint32_t)hbt.tgt.size();
     b.n_win = (uint32_t)hbt.win.size();
     b.n_ovl = (uint32_t)hbt.ovl.size();
     b.n_ow = (uint32_t)hbt.ow.size();
     b.batch_size = ctx->opt.batch_size;
-    b.rows_cap = L->rows_cap;
     b.n_raw = hbt.n_raw;
     b.op_base_dev = (uint32_t)hbt.op_cap;
-    set_view_ptrs(ctx, L, b);
     return b;
+}
+
+// Point the view at a row arena of at least `rows` rows, growing the row region if needed.  Its contents are not kept: every
+// attempt of a launch fills the row region anew.
+int set_rows(hb_ctx* ctx, hb_ctx::Lane* L, BatchView& b, uint64_t rows) {
+    if (rows > L->rows_cap) {
+        b.rows_cap = rows;
+        CK(L->d_rows.grow(carve_rows(b, nullptr)));
+        L->rows_cap = rows;
+    }
+    b.rows_cap = L->rows_cap;
+    carve_rows(b, L->d_rows.as<uint8_t>());
+    return HB_OK;
 }
 
 int zero_scratch(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b) {
@@ -707,12 +669,11 @@ int zero_scratch(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b) {
 }
 
 // The forward + consensus part once the number of supported positions is known.
-int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, uint64_t n_sup, uint64_t* launches) {
+int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, uint64_t n_sup, uint64_t* launches) {
     *launches += launch_features_c2(b, L->stream, L->kt);
     for (uint64_t n0 = 0; n0 < n_sup; n0 += ctx->chunk_pos) {
         const uint32_t np = (uint32_t)std::min<uint64_t>(ctx->chunk_pos, n_sup - n0);
-        *launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, np, L->d_ws.as<uint8_t>(), L->d_logits.as<float>(),
-                                          L->d_info.as<float>(), L->stream, L->kt);
+        *launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, np, f.ws, f.logits, f.info, L->stream, L->kt);
     }
     CK(cudaEventRecord(L->ev[4], L->stream));
     *launches += launch_consensus(b, L->stream, L->kt);
@@ -731,33 +692,37 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
     std::vector<Result> out_results;
     const uint32_t W = ctx->opt.window_size;
-    int rc = ensure_batch_buffers(ctx, L, hbt);
-    if (rc) return rc;
     const size_t nt = hbt.tgt.size(), nw = hbt.win.size();
+    // the regions may move below: the view kept from the lane's previous launch would point into freed memory
+    L->last.valid = false;
+    const size_t cig_bytes = hbt.cig.size();
+    const uint64_t op_slots = hbt.op_cap + hbt.dev_op_cap, raw_slots = hbt.raw_cap;
+    if (op_slots >= 0xffffffffull) return fail(ctx, HB_ERR_CAPACITY, "batch too large: more than 2^32 CIGAR ops (lower launch_targets)");
+    BatchView b = make_view(ctx, hbt);
+    CK(L->d_batch.grow(carve_batch(b, cig_bytes, op_slots, raw_slots, nullptr)));
+    carve_batch(b, cig_bytes, op_slots, raw_slots, L->d_batch.as<uint8_t>());
     // ---- H2D straight from the pinned staging arrays of the batch
     const size_t sz[5] = {vbytes(hbt.tgt), vbytes(hbt.win), vbytes(hbt.ovl), vbytes(hbt.ow), hbt.cig.size()};
     const void* src[5] = {hbt.tgt.data(), hbt.win.data(), hbt.ovl.data(), hbt.ow.data(), hbt.cig.data()};
-    void* dst[5] = {L->d_tgt.p, L->d_win.p, L->d_ovl.p, L->d_ow.p, L->d_cig.p};
+    void* dst[5] = {(void*)b.tgt, (void*)b.win, (void*)b.ovl, b.ow_mut, (void*)b.cig};
     for (int i = 0; i < 5; i++)
         if (sz[i]) CK(cudaMemcpyAsync(dst[i], src[i], sz[i], cudaMemcpyHostToDevice, L->stream));
     S.h2d_bytes += sz[0] + sz[1] + sz[2] + sz[3] + sz[4];
 
-    if (L->rows_cap == 0) {
-        const uint64_t per_win = ctx->arena_rows_per_win ? ctx->arena_rows_per_win : (uint64_t)W + W / 2;
-        rc = ensure_row_buffers(ctx, L, (uint64_t)nw * per_win + 64);
-        if (rc) return rc;
-    }
-    CK(L->pin_small.ensure(CNT_N * 4 + nw * 4 * 4 + nt * 4 + nw * TOP_K * 4 + 1024));
-    uint32_t* h_cnt = L->pin_small.as<uint32_t>();
+    // a lane's first launch starts with 1.5 W rows per window (HERRO_B200_ARENA_ROWS overrides); later ones keep their arena
+    const uint64_t per_win = ctx->arena_rows_per_win ? ctx->arena_rows_per_win : (uint64_t)W + W / 2;
+    int rc = set_rows(ctx, L, b, L->rows_cap ? L->rows_cap : (uint64_t)nw * per_win + 64);
+    if (rc) return rc;
+    Readback h;
+    CK(L->pin_small.grow(carve_readback(h, nt, nw, nullptr)));
+    carve_readback(h, nt, nw, L->pin_small.as<uint8_t>());
     uint64_t launches = 0;
-    BatchView b;
     uint64_t total_rows = 0;
     PHASE(0);
     L->kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
     L->kt.st = L->stream;
     for (int attempt = 0;; attempt++) {
         if (attempt) L->kt.discard();
-        b = make_view(ctx, L, hbt);
         rc = zero_scratch(ctx, L, b);
         if (rc) return rc;
         CK(cudaEventRecord(L->ev[0], L->stream));
@@ -766,49 +731,40 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
         CK(cudaEventRecord(L->ev[2], L->stream));
         launches += launch_features_c1(b, L->stream, L->kt);  // ref_lmax + scan; the work list needs its buffers first
-        CK(cudaMemcpyAsync(h_cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaMemcpyAsync(h.cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
         PHASE(1);
         SYNC_TIMED();
         PHASE(2);
-        total_rows = (uint64_t)h_cnt[CNT_TOTAL_ROWS] | ((uint64_t)h_cnt[CNT_TOTAL_ROWS + 1] << 32);
-        if (!h_cnt[CNT_OVERFLOW]) break;
+        total_rows = (uint64_t)h.cnt[CNT_TOTAL_ROWS] | ((uint64_t)h.cnt[CNT_TOTAL_ROWS + 1] << 32);
+        if (!h.cnt[CNT_OVERFLOW]) break;
         if (attempt >= 2) return fail(ctx, HB_ERR_CAPACITY, "row arena overflow persisted after regrowth");
-        rc = ensure_row_buffers(ctx, L, total_rows + total_rows / 8 + 4096);
+        rc = set_rows(ctx, L, b, total_rows + total_rows / 8 + 4096);
         if (rc) return rc;
     }
-    const uint64_t n_sup = (uint64_t)h_cnt[CNT_NSUP] | ((uint64_t)h_cnt[CNT_NSUP + 1] << 32);
-    CK(L->d_fwd_win.ensure(std::max<uint64_t>(n_sup, 1) * 4));
-    CK(L->d_fwd_row.ensure(std::max<uint64_t>(n_sup, 1) * 4));
-    CK(L->d_logits.ensure(std::max<uint64_t>(n_sup, 1) * 5 * 4));
-    CK(L->d_info.ensure(std::max<uint64_t>(n_sup, 1) * 4));
-    CK(L->d_ws.ensure(fwd_workspace_bytes(ctx->wt, (uint32_t)std::min<uint64_t>(ctx->chunk_pos, std::max<uint64_t>(n_sup, 1)))));
-    b = make_view(ctx, L, hbt);
+    const uint64_t n_sup = (uint64_t)h.cnt[CNT_NSUP] | ((uint64_t)h.cnt[CNT_NSUP + 1] << 32);
+    FwdBufs f;
+    CK(L->d_fwd.grow(carve_fwd(ctx, b, f, n_sup, nullptr)));
+    carve_fwd(ctx, b, f, n_sup, L->d_fwd.as<uint8_t>());
     CK(cudaEventRecord(L->ev[3], L->stream));
-    rc = launch_tail(ctx, L, b, n_sup, &launches);
+    rc = launch_tail(ctx, L, b, f, n_sup, &launches);
     if (rc) return rc;
 
     // ---- D2H: per-window metadata, then exactly the emitted bytes
-    uint32_t* h_outlen = h_cnt + CNT_N;
-    uint32_t* h_nsel = h_outlen + nw;
-    uint32_t* h_L = h_nsel + nw;
-    uint32_t* h_nsup = h_L + nw;
-    uint32_t* h_terr = h_nsup + nw;
-    uint32_t* h_sel = h_terr + nt;
-    CK(cudaMemcpyAsync(h_cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_outlen, b.w_outlen, nw * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_nsel, b.w_nsel, nw * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_L, b.w_L, nw * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_nsup, b.w_nsup, nw * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_terr, b.tgt_err, nt * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h_sel, b.sel_ow, nw * TOP_K * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.outlen, b.w_outlen, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.nsel, b.w_nsel, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.L, b.w_L, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.nsup, b.w_nsup, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.terr, b.tgt_err, nt * 4, cudaMemcpyDeviceToHost, L->stream));
+    CK(cudaMemcpyAsync(h.sel, b.sel_ow, nw * TOP_K * 4, cudaMemcpyDeviceToHost, L->stream));
     // the emitted bytes of all windows are contiguous from offset 0 and number at most one per matrix row, so the
     // row count (known since the first wait) bounds the copy: no second round trip for the exact size
-    CK(L->pin_out.ensure(total_rows + 16));
+    CK(L->pin_out.grow(total_rows + 16));
     if (total_rows) CK(cudaMemcpyAsync(L->pin_out.p, b.out_bytes, total_rows, cudaMemcpyDeviceToHost, L->stream));
     PHASE(3);
     SYNC_TIMED();
     PHASE(4);
-    const uint64_t total_out = (uint64_t)h_cnt[CNT_TOTAL_OUT] | ((uint64_t)h_cnt[CNT_TOTAL_OUT + 1] << 32);
+    const uint64_t total_out = (uint64_t)h.cnt[CNT_TOTAL_OUT] | ((uint64_t)h.cnt[CNT_TOTAL_OUT + 1] << 32);
     if (total_out > total_rows) return fail(ctx, HB_ERR_CAPACITY, "consensus emitted more bytes than matrix rows");
     S.d2h_bytes += CNT_N * 4 + nw * 16 + nt * 4 + nw * TOP_K * 4 + total_rows;
 
@@ -837,17 +793,17 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         Result r;
         r.rid = tg.rid;
         r.status = HB_OK;
-        if (h_terr[t] & TERR_BAD_INPUT) {
+        if (h.terr[t] & TERR_BAD_INPUT) {
             r.status = HB_ERR_INPUT;
             r.msg = "input the reference would panic on (malformed CIGAR / window descriptor / query coordinates)";
-        } else if (h_terr[t] & TERR_TOO_MANY_COLS) {
+        } else if (h.terr[t] & TERR_TOO_MANY_COLS) {
             r.status = HB_ERR_CAPACITY;
             r.msg = "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window";
         }
         std::vector<uint8_t> cur;
         for (uint32_t w = tg.win_begin; w < tg.win_end; w++) {
-            const uint32_t len = h_outlen[w];
-            if (h_nsel[w] >= 2) {
+            const uint32_t len = h.outlen[w];
+            if (h.nsel[w] >= 2) {
                 cur.insert(cur.end(), outb + o, outb + o + len);
             } else if (!cur.empty()) {
                 r.seg_len.push_back((uint32_t)cur.size());
@@ -859,13 +815,13 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
             // 31 columns the kernel consumes)
             const DevWin& dw = hbt.win[w];
             uint64_t cb = 0;
-            for (uint32_t c = 0; c < h_nsel[w]; c++) {
-                const DevOW& ow = hbt.ow[h_sel[(size_t)w * TOP_K + c]];
+            for (uint32_t c = 0; c < h.nsel[w]; c++) {
+                const DevOW& ow = hbt.ow[h.sel[(size_t)w * TOP_K + c]];
                 const DevOverlap& ov = hbt.ovl[ow.ovl];
                 if (ov.raw_base == RAW_NONE) cb += ow.cei - ow.csi;
                 else cb += (uint64_t)ov.cig_len * W / std::max<uint32_t>(ov.tend - ov.tstart, W);  // device-windowed: its share of the CIGAR
             }
-            algo += (uint64_t)(h_nsel[w] + 1) * ((dw.len + 3) / 4 + dw.len) + cb + 2ull * R_COLS * h_L[w];
+            algo += (uint64_t)(h.nsel[w] + 1) * ((dw.len + 3) / 4 + dw.len) + cb + 2ull * R_COLS * h.L[w];
         }
         if (!cur.empty()) {
             r.seg_len.push_back((uint32_t)cur.size());
@@ -890,15 +846,15 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     LastLaunch ll;
     ll.valid = true;
     ll.win.assign(hbt.win.begin(), hbt.win.end());
-    ll.w_L.assign(h_L, h_L + nw);
-    ll.w_nsel.assign(h_nsel, h_nsel + nw);
-    ll.w_nsup.assign(h_nsup, h_nsup + nw);
+    ll.w_L.assign(h.L, h.L + nw);
+    ll.w_nsel.assign(h.nsel, h.nsel + nw);
+    ll.w_nsup.assign(h.nsup, h.nsup + nw);
     ll.w_rowbase.resize(nw);
     ll.w_supbase.resize(nw);
     uint64_t rb = 0, sb = 0;
     for (size_t w = 0; w < nw; w++) {
-        ll.w_rowbase[w] = rb; rb += h_L[w];
-        ll.w_supbase[w] = sb; sb += h_nsup[w];
+        ll.w_rowbase[w] = rb; rb += h.L[w];
+        ll.w_supbase[w] = sb; sb += h.nsup[w];
         if (ctx->opt.flags & HB_FLAG_KEEP_DEBUG) ll.index[((uint64_t)hbt.win[w].rid << 32) | hbt.win[w].wid] = (uint32_t)w;
     }
     if (ctx->opt.flags & HB_FLAG_KEEP_DEBUG) {
@@ -907,7 +863,11 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     }
     ll.n_sup = n_sup;
     ll.total_rows = total_rows;
+    ll.cig_bytes = cig_bytes;
+    ll.op_slots = op_slots;
+    ll.raw_slots = raw_slots;
     ll.view = b;
+    ll.fwd = f;
     S.ms_worker_busy = now_ms() - t_begin;
     S.ms_worker_gpu_wait = t_wait;
     {
@@ -1014,31 +974,35 @@ hb_ctx::ThreadSlot* my_slot(hb_ctx* ctx) {
 
 // Record the capacities this lane ended up with; other lanes grow to them while idle (see hb_ctx::LaneSizes).  Lock held.
 void publish_lane_sizes(hb_ctx* ctx, hb_ctx::Lane* L) {
-    DevBuf* bufs[hb_ctx::Lane::N_DEV];
-    L->all_bufs(bufs);
-    bool grew = false;
+    bool grew = false, below = false;
     hb_ctx::LaneSizes& T = ctx->lane_sizes;
-    for (int i = 0; i < hb_ctx::Lane::N_DEV; i++)
-        if (bufs[i]->cap > T.dev[i]) { T.dev[i] = bufs[i]->cap; grew = true; }
-    if (L->pin_small.cap > T.pin_small) { T.pin_small = L->pin_small.cap; grew = true; }
-    if (L->pin_out.cap > T.pin_out) { T.pin_out = L->pin_out.cap; grew = true; }
-    if (L->rows_cap > T.rows_cap) { T.rows_cap = L->rows_cap; grew = true; }
+    auto track = [&](size_t& t, size_t have) {
+        if (have > t) { t = have; grew = true; }
+        below = below || have < t;
+    };
+    track(T.batch, L->d_batch.cap);
+    track(T.rows, L->d_rows.cap);
+    track(T.fwd, L->d_fwd.cap);
+    track(T.pin_small, L->pin_small.cap);
+    track(T.pin_out, L->pin_out.cap);
+    track(T.rows_cap, L->rows_cap);
     if (grew) ctx->lane_sizes_version++;
-    bool below = L->pin_small.cap < T.pin_small || L->pin_out.cap < T.pin_out || L->rows_cap < T.rows_cap;
-    for (int i = 0; i < hb_ctx::Lane::N_DEV; i++) below = below || bufs[i]->cap < T.dev[i];
     if (!below) L->seen_sizes = ctx->lane_sizes_version;  // else: this lane catches up when it is next idle
 }
 
-// Grow an idle lane's buffers to the recorded sizes (no lock held; only this lane's worker touches its buffers).
+// Grow an idle lane's regions to the recorded sizes (no lock held; only this lane's worker touches its regions).
 void presize_lane(hb_ctx* ctx, hb_ctx::Lane* L, const hb_ctx::LaneSizes& T) {
-    DevBuf* bufs[hb_ctx::Lane::N_DEV];
-    L->all_bufs(bufs);
-    bool ok = true;
-    for (int i = 0; i < hb_ctx::Lane::N_DEV; i++) ok = ok && bufs[i]->reserve_exact(T.dev[i]) == cudaSuccess;
-    ok = ok && L->pin_small.reserve_exact(T.pin_small) == cudaSuccess && L->pin_out.reserve_exact(T.pin_out) == cudaSuccess;
-    if (ok && T.rows_cap > L->rows_cap) L->rows_cap = T.rows_cap;  // the six row-sized buffers are part of dev[]
+    const bool ok = L->d_batch.grow(T.batch, false, true) == cudaSuccess && L->d_rows.grow(T.rows, false, true) == cudaSuccess &&
+                    L->d_fwd.grow(T.fwd, false, true) == cudaSuccess && L->pin_small.grow(T.pin_small, false) == cudaSuccess &&
+                    L->pin_out.grow(T.pin_out, false) == cudaSuccess;
+    if (ok && T.rows_cap > L->rows_cap) L->rows_cap = T.rows_cap;  // T.rows holds a row arena of T.rows_cap rows
     cudaStreamSynchronize(L->stream);
-    if (L->last.valid) set_view_ptrs(ctx, L, L->last.view);  // buffers moved (contents copied): the kept view follows them
+    LastLaunch& ll = L->last;
+    if (ll.valid) {  // the regions moved with their contents: carving the kept view's counts again gives the same offsets
+        carve_batch(ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, L->d_batch.as<uint8_t>());
+        carve_rows(ll.view, L->d_rows.as<uint8_t>());
+        carve_fwd(ctx, ll.view, ll.fwd, ll.n_sup, L->d_fwd.as<uint8_t>());
+    }
 }
 
 
@@ -1322,7 +1286,7 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         if (cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
         for (auto& e : L.ev)
             if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
-        L.bind_stream();
+        L.d_batch.st = L.d_rows.st = L.d_fwd.st = L.stream;
     }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
         cudaMemPool_t pool;
@@ -1380,18 +1344,18 @@ int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_wo
     // Padded on both sides: packed 32-base extraction may touch a few words past a read, and the pileup kernel fetches the
     // 4 bases / 4 quality bytes of a row group as whole words that may start up to 7 bytes before a read (pileup.cu).
     constexpr size_t FRONT_WORDS = 32, FRONT_QUAL = 256;  // keeps both bases 256-byte aligned
-    CK(ctx->d_words.ensure((FRONT_WORDS + woff[n_reads] + 8) * 8));
+    CK(ctx->d_words.grow((FRONT_WORDS + woff[n_reads] + 8) * 8));
     CK(cudaMemset(ctx->d_words.p, 0, FRONT_WORDS * 8));
     CK(cudaMemset(ctx->d_words.as<uint64_t>() + FRONT_WORDS + woff[n_reads], 0, 8 * 8));
-    CK(ctx->d_qual.ensure(FRONT_QUAL + qoff[n_reads] + 16));
+    CK(ctx->d_qual.grow(FRONT_QUAL + qoff[n_reads] + 16));
     CK(cudaMemset(ctx->d_qual.p, 33, FRONT_QUAL));
     CK(cudaMemset(ctx->d_qual.as<uint8_t>() + FRONT_QUAL + qoff[n_reads], 33, 16));
-    CK(ctx->d_word_off.ensure((n_reads + 1) * 8));
-    CK(ctx->d_qual_off.ensure((n_reads + 1) * 8));
-    CK(ctx->d_len.ensure((size_t)n_reads * 4));
+    CK(ctx->d_word_off.grow((n_reads + 1) * 8));
+    CK(ctx->d_qual_off.grow((n_reads + 1) * 8));
+    CK(ctx->d_len.grow((size_t)n_reads * 4));
     // stage in pinned chunks
     const size_t CH = 64u << 20;
-    CK(ctx->pin_in.ensure(CH));
+    CK(ctx->pin_in.grow(CH));
     uint8_t* pin = ctx->pin_in.as<uint8_t>();
     auto copy_stream = [&](auto getp, auto getn, uint8_t* dbase) -> int {
         size_t fill = 0, doff = 0;
@@ -1425,7 +1389,7 @@ int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_wo
     std::vector<double> ln(ctx->ln_n);
     ln[0] = 0.0;
     for (uint32_t k = 1; k < ctx->ln_n; k++) ln[k] = std::log((double)k);
-    CK(ctx->d_ln.ensure((size_t)ctx->ln_n * 8));
+    CK(ctx->d_ln.grow((size_t)ctx->ln_n * 8));
     CK(cudaMemcpy(ctx->d_ln.p, ln.data(), (size_t)ctx->ln_n * 8, cudaMemcpyHostToDevice));
     ctx->stats.h2d_bytes += woff[n_reads] * 8 + qoff[n_reads];
     ctx->n_reads = n_reads;
@@ -1669,8 +1633,8 @@ int hb_debug_dump_window(hb_ctx* ctx, uint32_t rid, uint32_t wid, uint8_t* bases
             for (uint32_t k = 0; k < ns; k++) { supported[2 * k] = (t[k] >> 8) & 0xffffu; supported[2 * k + 1] = t[k] & 0xffu; }
         }
         if (sup_rows) CK(cudaMemcpy(sup_rows, ll.view.sup_row + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-        if (info_logits) CK(cudaMemcpy(info_logits, lane->d_info.as<float>() + sb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-        if (bases_logits) CK(cudaMemcpy(bases_logits, lane->d_logits.as<float>() + sb * 5, (size_t)ns * 20, cudaMemcpyDeviceToHost));
+        if (info_logits) CK(cudaMemcpy(info_logits, ll.fwd.info + sb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+        if (bases_logits) CK(cudaMemcpy(bases_logits, ll.fwd.logits + sb * 5, (size_t)ns * 20, cudaMemcpyDeviceToHost));
     }
     return HB_OK;
 }
@@ -1873,7 +1837,7 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
         launches += launch_features_a(b, L->stream, L->kt);
         launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
         launches += launch_features_c1(b, L->stream, L->kt);
-        rc = launch_tail(ctx, L, b, L->last.n_sup, &launches);
+        rc = launch_tail(ctx, L, b, L->last.fwd, L->last.n_sup, &launches);
         if (rc) return rc;
     }
     CK(cudaEventRecord(L->ev[7], L->stream));

@@ -318,7 +318,6 @@ __global__ void k_heads(BatchView b, FwdWeights wt, uint32_t n0, uint32_t npos, 
 }
 
 // ------------------------------------------------------------------------------------------
-static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 struct FwdWs {
     float *X, *QKV, *Z;
     __nv_bfloat16 *Hhi, *Hlo, *Fhi, *Flo;

@@ -134,6 +134,9 @@ struct KTimer {
 enum { K_TOKENIZE = 0, K_PASS1, K_SCORES, K_PASS2A, K_SCAN, K_PILEUP, K_LISTS, K_STEM, K_LAYERNORM, K_GEMM, K_ATTENTION,
        K_HEADS, K_CONSENSUS, K_FFN, K_QKV_ATTN };
 
+// Scratch is carved from one allocation into arrays that each start 256-byte aligned, the alignment a separate cudaMalloc
+// would give: TMA operands and 16-byte row stores rely on it.
+inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 size_t fwd_workspace_bytes(const FwdWeights& wt, uint32_t chunk_pos);
 int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, uint32_t npos, uint8_t* ws,
                          float* logits, float* info, cudaStream_t st, KTimer& kt);
