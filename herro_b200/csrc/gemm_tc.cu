@@ -14,8 +14,9 @@
 //   k_ffn_ws       FFN1 -> ReLU -> FFN2 + residual + LayerNorm, hidden activations kept on chip
 //   k_qkv_attn_ws  QKV projection (wgmma) + per-position attention (mma.sync)
 //   k_stem_tc      embedding + conv stem as a contraction, A tile synthesised from the pileup matrix, + first LayerNorm
-// Common skeleton: two consumer warpgroups (warps 0-7) and one producer warp (warp 8, one lane issues TMA into a ring of
-// k-block stages guarded by full / empty mbarriers).  A work item is a tile of 128 rows; consumer warpgroup wg issues
+// Common skeleton: two consumer warpgroups (warps 0-7) and one producer warp (warp 8; k_ffn_ws: producer warpgroup, warps 8-11),
+// one lane of which issues TMA into a ring of k-block stages guarded by full / empty mbarriers.  A work item is a tile of 128
+// rows; consumer warpgroup wg issues
 // wgmma.m64nNk16 for rows [64 wg, 64 wg + 64) and runs the epilogue on its own accumulator fragments:
 // thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 and that + 8, columns 8 j + 2 (t % 4) + {0, 1}
 // (acc[4 j], acc[4 j + 1] for the first row, acc[4 j + 2], acc[4 j + 3] for the second).  A row's 128 columns live in
@@ -104,6 +105,18 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint6
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
+// D[64 x 128] += A[64 x 16] · B[128 x 16]^T, A from registers, B K-major in shared memory.  The A fragment of the warpgroup's
+// thread t is the accumulator layout above restricted to 16 columns: a0 = row r, columns 2 (t % 4) + {0, 1}; a1 = row r + 8;
+// a2, a3 = the same rows 8 columns on (bf16 pairs, lower column in the low half)
+__device__ __forceinline__ void wgmma_n128_ra(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc)
+        : "memory");
+}
 // D[64 x 96] (+)= A[64 x 16] · B[96 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulator in registers
 __device__ __forceinline__ void wgmma_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
@@ -128,6 +141,28 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[64], uint32_t a_hi, uint
         wgmma_n128(acc, dAh + adv, dBl + adv, 1u);
     }
     wg_commit();
+}
+// the same with A from registers: ah / al hold a 128-wide k range as 8 k-slices of 4 fragment registers; k-block kb is
+// slices 4 kb .. 4 kb + 3.  Same pass order as mma_kblock.
+__device__ __forceinline__ void mma_kblock_ra(float (&acc)[64], const uint32_t (&ah)[32], const uint32_t (&al)[32], int kb, uint32_t b_hi,
+                                              uint32_t b_lo) {
+    const uint64_t dBh = make_desc(b_hi), dBl = make_desc(b_lo);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; k++) {
+        const uint64_t adv = (uint64_t)(k * 2);
+        const int s = 4 * (4 * kb + k);
+        wgmma_n128_ra(acc, ah[s], ah[s + 1], ah[s + 2], ah[s + 3], dBh + adv);
+        wgmma_n128_ra(acc, al[s], al[s + 1], al[s + 2], al[s + 3], dBh + adv);
+        wgmma_n128_ra(acc, ah[s], ah[s + 1], ah[s + 2], ah[s + 3], dBl + adv);
+    }
+    wg_commit();
+}
+// keeps the compiler from reusing A fragment registers that an in-flight wgmma still reads
+template <int R>
+__device__ __forceinline__ void reg_fence(uint32_t (&a)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -321,11 +356,16 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_ws(GemmArgs g, const __gr
 // The hidden activations never leave the SM: per 128-token tile and per 128-wide hidden chunk c, each consumer warpgroup
 // (64 rows) runs
 //   F1(c): accF = H · W1[c]^T           (H tile resident in shared memory)
-//   E1(c): relu(accF + b1[c]) -> split bf16 -> the warpgroup's rows of the swizzled K-major tile A2 in shared memory
-//   F2(c): accO += A2 · W2[:, c]^T
+//   E1(c): relu(accF + b1[c]) -> split bf16 -> A fragments in registers: the accumulator layout is the A fragment layout of
+//          the next contraction, k-slice s being (accF[8s], accF[8s+1]), (accF[8s+2], accF[8s+3]), ..., (accF[8s+6], accF[8s+7])
+//   F2(c): accO += A · W2[:, c]^T       (wgmma with A from registers)
 // accO starts as X + b2, so after F2(3) it holds the new residual row: one final epilogue stores it and its LayerNorm.
-// W k-block tiles stream through the TMA ring in issue order F1(0) F2(0) F1(1) F2(1) ... F2(3).  Saves writing and
-// re-reading the [T, F] hidden tensor (4 KB per token and layer).
+// Issue order per warpgroup: F1(0) E1(0) [F2(0) F1(1)] E1(1) ... [F2(2) F1(3)] E1(3) F2(3).  F2(c) and F1(c+1) are issued
+// back to back; F2(c) was issued first, so once F1(c+1) has completed the A fragments may be overwritten.  Live registers:
+// accO 64 + accF 64 + A fragments 64, within the 240 that setmaxnreg gives each consumer thread.
+// W k-block tiles stream through the TMA ring in issue order F1(0) F2(0) F1(1) F2(1) ... F2(3).  Every k-block is one wgmma
+// group and its stage is freed as soon as that group has completed, so the producer runs up to FFN_STAGES k-blocks ahead,
+// across contractions and tiles.  Saves writing and re-reading the [T, F] hidden tensor (4 KB per token and layer).
 // FUSE_O: the attention out-projection, its residual add and LayerNorm (ln2) run in front of the FFN inside this kernel:
 //   P0   : accO = O · Wo^T                       (O = attention output tile, loaded where H used to be)
 //   E0   : accO = accO + bo + X (= X'), H = LN2(X') -> split bf16 -> written over the warpgroup's rows of the O tile
@@ -334,10 +374,23 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_ws(GemmArgs g, const __gr
 // ------------------------------------------------------------------------------------------------
 constexpr int FFN_RING_BYTES = 2 * BN * 128;        // one W k-block tile, hi + lo: 32 KB
 constexpr int FFN_A_BYTES = 2 * 2 * BM * 128;       // a [128 x 128] operand as 2 k-blocks x (hi, lo): 64 KB
-constexpr int FFN_STAGES = 2;                       // 2 x 64 KB operand tiles + 2 x 32 KB ring = 192 KB
+constexpr int FFN_STAGES = 4;                       // 64 KB operand tile + 4 x 32 KB ring = 192 KB
+// consumers: warps 0-7 (two warpgroups); producer: warpgroup 2 (warps 8-11), one lane of which issues the TMA.  setmaxnreg
+// moves registers from the producer to the consumers: 24 x 128 + 240 x 256 <= 65 536.  The producer loop fits in 24; with
+// 232 per consumer, FUSE_O spills loop state.
+constexpr int FFN_THREADS = 384, FFN_PROD_WARP = 8, FFN_PROD_REGS = 24, FFN_CONS_REGS = 240;
+
+// waits for the in-flight k-block groups oldest first and frees each one's ring stage as soon as it has completed;
+// it_stage counts the k-blocks issued so far
+template <int N>
+__device__ __forceinline__ void ffn_retire(uint64_t* empty_bar, uint32_t it_stage) {
+    wg_wait<N>();
+    mbar_arrive(&empty_bar[(it_stage - 1 - N) % FFN_STAGES]);
+    if constexpr (N > 0) ffn_retire<N - 1>(empty_bar, it_stage);
+}
 
 template <bool FUSE_O>
-__global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid_constant__ CUtensorMap tmHhi,
+__global__ void __launch_bounds__(FFN_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid_constant__ CUtensorMap tmHhi,
                                                         const __grid_constant__ CUtensorMap tmHlo, const __grid_constant__ CUtensorMap tmW1hi,
                                                         const __grid_constant__ CUtensorMap tmW1lo, const __grid_constant__ CUtensorMap tmW2hi,
                                                         const __grid_constant__ CUtensorMap tmW2lo, const __grid_constant__ CUtensorMap tmWohi,
@@ -345,8 +398,7 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
     uint8_t* sA1 = smem;                            // H tile: [kb][hi|lo][128 x 128 B]
-    uint8_t* sA2 = sA1 + FFN_A_BYTES;               // relu(hidden chunk) tile, same layout
-    uint8_t* ring = sA2 + FFN_A_BYTES;              // FFN_STAGES x FFN_RING_BYTES
+    uint8_t* ring = sA1 + FFN_A_BYTES;              // FFN_STAGES x FFN_RING_BYTES
     __shared__ uint64_t full_bar[FFN_STAGES], empty_bar[FFN_STAGES], a1_full, a1_empty;
     __shared__ __align__(16) float s_b1[512], s_b2[BN], s_lng[BN], s_lnb[BN], s_bo[BN], s_ln2g[BN], s_ln2b[BN];
 
@@ -356,14 +408,15 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid
         mbar_init(&a1_full, 1); mbar_init(&a1_empty, C_THREADS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = tid; i < 512; i += G_THREADS) s_b1[i] = g.b1[i];
+    for (int i = tid; i < 512; i += FFN_THREADS) s_b1[i] = g.b1[i];
     if (tid < BN) { s_b2[tid] = g.b2[tid]; s_lng[tid] = g.ln_g[tid]; s_lnb[tid] = g.ln_b[tid]; }
     if (FUSE_O && tid < BN) { s_bo[tid] = g.bo[tid]; s_ln2g[tid] = g.ln2_g[tid]; s_ln2b[tid] = g.ln2_b[tid]; }
     __syncthreads();
 
-    if (warp == G_PROD_WARP) {
+    if (warp >= FFN_PROD_WARP) {
         // =============================== producer: one lane issues the TMA copies ===============================
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(FFN_PROD_REGS));
+        if (warp == FFN_PROD_WARP && lane == 0) {
             uint32_t it_stage = 0, n_done = 0;
             auto load_w = [&](const CUtensorMap* hi, const CUtensorMap* lo, int col, int row) {
                 const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
@@ -394,32 +447,54 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid
         return;
     }
     // =============================== consumers ===============================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(FFN_CONS_REGS));
     const int wg = warp >> 2;
     const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2), fc = (lane & 3) * 2;
-    const uint32_t a1b = smem_u32(sA1) + wg * 64 * 128, a2b = smem_u32(sA2) + wg * 64 * 128;  // this warpgroup's rows
+    const uint32_t a1b = smem_u32(sA1) + wg * 64 * 128;  // this warpgroup's rows of the resident tile
     uint32_t it_stage = 0, n_done = 0;
     float accO[64], accF[64];
-    // two k-blocks of A (resident tile at abase) against the next two ring stages
-    auto contract = [&](float (&acc)[64], uint32_t abase, bool zero) {
+    uint32_t ahi[32], alo[32];  // relu(hidden chunk) as split bf16 A fragments of F2
+    // k-block kb of the resident tile against the next ring stage, one wgmma group
+    auto issue = [&](float (&acc)[64], int kb, bool zero) {
+        const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES), a = a1b + kb * (2 * BM * 128);
+        mma_kblock(acc, a, a + BM * 128, sb, sb + BN * 128, zero && kb == 0);
+        it_stage++;
+    };
+    // F2(c): k-blocks 0, 1 of the A fragments against the next two ring stages
+    auto issue_f2 = [&]() {
+#pragma unroll
         for (int kb = 0; kb < 2; kb++, it_stage++) {
             const uint32_t s = it_stage % FFN_STAGES, ph = (it_stage / FFN_STAGES) & 1;
             mbar_wait(&full_bar[s], ph);
             const uint32_t sb = smem_u32(ring + (size_t)s * FFN_RING_BYTES);
-            const uint32_t a = abase + kb * (2 * BM * 128);
-            mma_kblock(acc, a, a + BM * 128, sb, sb + BN * 128, zero && kb == 0);
+            mma_kblock_ra(accO, ahi, alo, kb, sb, sb + BN * 128);
         }
-        wg_wait<0>();
-        acc_fence(acc);
-        mbar_arrive(&empty_bar[(it_stage - 2) % FFN_STAGES]);
-        mbar_arrive(&empty_bar[(it_stage - 1) % FFN_STAGES]);
+    };
+    // E1(c): relu(accF + b1[c]) -> split bf16 A fragments
+    auto e1 = [&](int c) {
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const float b0 = s_b1[c * 128 + 8 * j + fc], b1 = s_b1[c * 128 + 8 * j + fc + 1];
+            split2(fmaxf(accF[4 * j] + b0, 0.f), fmaxf(accF[4 * j + 1] + b1, 0.f), ahi[2 * j], alo[2 * j]);
+            split2(fmaxf(accF[4 * j + 2] + b0, 0.f), fmaxf(accF[4 * j + 3] + b1, 0.f), ahi[2 * j + 1], alo[2 * j + 1]);
+        }
     };
     for (uint32_t tile = blockIdx.x; tile < g.m_tiles; tile += gridDim.x, n_done++) {
         const size_t row0 = (size_t)tile * BM + fr;
+        // the residual rows X, loaded before the first wait so that their latency hides behind the tile's TMA (and P0)
+        float2 xr[32];
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            xr[2 * j] = *(const float2*)(g.X + row0 * BN + 8 * j + fc);
+            xr[2 * j + 1] = *(const float2*)(g.X + (row0 + 8) * BN + 8 * j + fc);
+        }
         if (!FUSE_O) {  // accO = X + b2: the FFN2 contractions accumulate on top of the residual row
 #pragma unroll
             for (int j = 0; j < 16; j++) {
                 const int c = 8 * j + fc;
-                const float2 x0 = *(const float2*)(g.X + row0 * BN + c), x1 = *(const float2*)(g.X + (row0 + 8) * BN + c);
+                const float2 x0 = xr[2 * j], x1 = xr[2 * j + 1];
                 accO[4 * j] = x0.x + s_b2[c]; accO[4 * j + 1] = x0.y + s_b2[c + 1];
                 accO[4 * j + 2] = x1.x + s_b2[c]; accO[4 * j + 3] = x1.y + s_b2[c + 1];
             }
@@ -427,11 +502,14 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid
         mbar_wait(&a1_full, n_done & 1);
         if (FUSE_O) {
             // ---- P0 + E0: X' = O · Wo^T + bo + X;  H = LN2(X') over this warpgroup's rows of the O tile
-            contract(accO, a1b, true);
+            issue(accO, 0, true);
+            issue(accO, 1, true);
+            ffn_retire<1>(empty_bar, it_stage);
+            acc_fence(accO);
 #pragma unroll
             for (int j = 0; j < 16; j++) {
                 const int c = 8 * j + fc;
-                const float2 x0 = *(const float2*)(g.X + row0 * BN + c), x1 = *(const float2*)(g.X + (row0 + 8) * BN + c);
+                const float2 x0 = xr[2 * j], x1 = xr[2 * j + 1];
                 accO[4 * j] = accO[4 * j] + s_bo[c] + x0.x; accO[4 * j + 1] = accO[4 * j + 1] + s_bo[c + 1] + x0.y;
                 accO[4 * j + 2] = accO[4 * j + 2] + s_bo[c] + x1.x; accO[4 * j + 3] = accO[4 * j + 3] + s_bo[c + 1] + x1.y;
             }
@@ -447,21 +525,27 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_ffn_ws(FfnArgs g, const __grid
             fence_async_smem();
             bar_sync(1 + wg, 128);  // the warpgroup's H rows are complete before its FFN1 reads them
         }
-        for (int c = 0; c < 4; c++) {
-            contract(accF, a1b, true);                                 // F1(c)
-            if (c == 3) mbar_arrive(&a1_empty);                        // the H tile is no longer needed
-#pragma unroll
-            for (int j = 0; j < 16; j++) {                             // E1(c)
-                const float b0 = s_b1[c * 128 + 8 * j + fc], b1 = s_b1[c * 128 + 8 * j + fc + 1];
-                accF[4 * j] = fmaxf(accF[4 * j] + b0, 0.f); accF[4 * j + 1] = fmaxf(accF[4 * j + 1] + b1, 0.f);
-                accF[4 * j + 2] = fmaxf(accF[4 * j + 2] + b0, 0.f); accF[4 * j + 3] = fmaxf(accF[4 * j + 3] + b1, 0.f);
-            }
-            frag_store_tile(accF, sA2, fr, fc);
-            fence_async_smem();
-            bar_sync(1 + wg, 128);
-            contract(accO, a2b, false);                                // F2(c)
-            bar_sync(1 + wg, 128);                                     // F2(c) has read A2 before the next E1 overwrites it
+        issue(accF, 0, true);                                          // F1(0)
+        issue(accF, 1, true);
+        ffn_retire<1>(empty_bar, it_stage);
+        acc_fence(accF);
+        e1(0);
+        for (int c = 0; c < 3; c++) {
+            issue_f2();                                                // F2(c)
+            issue(accF, 0, true);                                      // F1(c+1)
+            issue(accF, 1, true);
+            ffn_retire<3>(empty_bar, it_stage);
+            acc_fence(accF);
+            reg_fence(ahi);
+            reg_fence(alo);
+            if (c == 2) mbar_arrive(&a1_empty);                        // the H tile is no longer needed
+            e1(c + 1);
         }
+        issue_f2();                                                    // F2(3)
+        ffn_retire<1>(empty_bar, it_stage);
+        acc_fence(accO);
+        reg_fence(ahi);
+        reg_fence(alo);
         // ---- final epilogue: X = accO (residual already in); LayerNorm -> split bf16
         if (g.store_x) frag_store_f32(accO, g.X, BN, row0, 0, fc);
         frag_layernorm(accO, s_lng, s_lnb, fc);
@@ -976,7 +1060,7 @@ cudaError_t gemm_tc(const GemmArgs& a, int num_sms, cudaStream_t st) {
 
 cudaError_t ffn_tc(const FfnArgs& a, int num_sms, cudaStream_t st) {
     static bool configured = false;
-    const size_t smem = (size_t)2 * FFN_A_BYTES + (size_t)FFN_STAGES * FFN_RING_BYTES + 1024;
+    const size_t smem = (size_t)FFN_A_BYTES + (size_t)FFN_STAGES * FFN_RING_BYTES + 1024;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(k_ffn_ws<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -993,9 +1077,9 @@ cudaError_t ffn_tc(const FfnArgs& a, int num_sms, cudaStream_t st) {
     const unsigned grid = (unsigned)std::min<uint32_t>(a.m_tiles, (uint32_t)num_sms);
     if (a.Wohi) {
         if (!make_tmap(&toh, a.Wohi, BN, BN, BN) || !make_tmap(&tol, a.Wolo, BN, BN, BN)) return cudaErrorInvalidValue;
-        k_ffn_ws<true><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, toh, tol);
+        k_ffn_ws<true><<<grid, FFN_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, toh, tol);
     } else {
-        k_ffn_ws<false><<<grid, G_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, t1h, t1l);
+        k_ffn_ws<false><<<grid, FFN_THREADS, smem, st>>>(a, tHh, tHl, t1h, t1l, t2h, t2l, t1h, t1l);
     }
     return cudaGetLastError();
 }
