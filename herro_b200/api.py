@@ -38,7 +38,7 @@ class HbOptions(C.Structure):
 
 
 KERNEL_CLASSES = ["tokenize", "pass1", "scores", "pass2a", "scan", "pileup", "lists", "stem", "layernorm", "gemm",
-                  "attention", "heads", "consensus", "ffn", "qkv_attn"]
+                  "attention", "heads", "consensus", "ffn", "qkv_attn", "pos_attn"]
 
 
 class HbStats(C.Structure):
@@ -99,15 +99,18 @@ def load_library():
     L.hb_replay_last_launch.argtypes = [vp, u32, C.POINTER(C.c_float)]
     L.hb_dump_features.argtypes = [vp, u32, C.c_char_p, vp]
     L.hb_inspect_model.argtypes = [C.c_char_p, u32p, C.POINTER(C.c_uint64), C.c_char_p, C.c_size_t]
+    L.hb_inspect_model_ex.argtypes = [C.c_char_p, u32p, C.POINTER(C.c_uint64), C.c_char_p, C.c_size_t]
     fp = C.POINTER(C.c_float)
     L.hb_selftest_gemm.argtypes = [C.c_int, u32, u32, u32, C.c_int, C.c_int, u32, fp, fp, fp, fp]
+    L.hb_selftest_pos_attention.argtypes = [C.c_int, u32p, u32, u32, u32, fp, fp, fp]
     _lib = L
     return L
 
 
 EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "hb_bind_calling_thread", "hb_set_launch_targets", "hb_set_kernel_timing", "hb_extract_windows", "hb_create", "hb_destroy", "hb_upload_reads", "hb_submit_target", "hb_submit_alignments", "hb_flush",
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
-                    "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm"]
+                    "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
+                    "hb_inspect_model_ex", "hb_selftest_pos_attention"]
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
@@ -118,6 +121,25 @@ def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
     if rc != 0:
         raise HerroError(rc, L.hb_last_error(None).decode())
     return dict(max_abs_err=v[0].value, max_abs_ref=v[1].value, ms_tc=v[2].value, ms_simt=v[3].value)
+
+
+def selftest_pos_attention(lens, heads: int, head_dim: int, qkv: np.ndarray, device=0):
+    """The position-axis stage's masked attention kernel on sequences of `lens` rows stored back to back in `qkv`
+    ([sum lens, 3 * heads * head_dim] fp32, q | k | v) -> (output [sum lens, heads * head_dim] fp32, kernel ms)."""
+    L = load_library()
+    lens = np.ascontiguousarray(lens, dtype=np.uint32)
+    D = heads * head_dim
+    qkv = np.ascontiguousarray(qkv, dtype=np.float32)
+    if qkv.shape != (int(lens.sum()), 3 * D):
+        raise ValueError(f"qkv must be [{int(lens.sum())}, {3 * D}], got {qkv.shape}")
+    out = np.zeros((int(lens.sum()), D), dtype=np.float32)
+    ms = C.c_float()
+    fp = C.POINTER(C.c_float)
+    rc = L.hb_selftest_pos_attention(device, lens.ctypes.data_as(C.POINTER(C.c_uint32)), len(lens), heads, head_dim,
+                                     qkv.ctypes.data_as(fp), out.ctypes.data_as(fp), C.byref(ms))
+    if rc != 0:
+        raise HerroError(rc, L.hb_last_error(None).decode())
+    return out, ms.value
 
 
 # ------------------------------------------------------------------------------------------
@@ -157,15 +179,16 @@ def extract_windows(overlaps: np.ndarray, window_size: int, n_windows: int) -> n
 
 
 def inspect_model(path: str):
-    """Architecture and parameter hash of a model file (HB200W1 blob or TorchScript archive), host only (hb_inspect_model)."""
+    """Architecture and parameter hash of a model file (HB200W1 blob or TorchScript archive), host only (hb_inspect_model_ex)."""
     L = load_library()
-    dims = (C.c_uint32 * 6)()
+    dims = (C.c_uint32 * 9)()
     h = C.c_uint64()
     err = C.create_string_buffer(512)
-    rc = L.hb_inspect_model(path.encode(), dims, C.byref(h), err, len(err))
+    rc = L.hb_inspect_model_ex(path.encode(), dims, C.byref(h), err, len(err))
     if rc != 0:
         raise HerroError(rc, err.value.decode(errors="replace"))
-    return dict(zip(("stem_k", "channels", "heads", "layers", "ffn", "collapse"), [int(x) for x in dims])), int(h.value)
+    keys = ("stem_k", "channels", "heads", "layers", "ffn", "collapse", "pos_layers", "pos_heads", "pos_ffn")
+    return dict(zip(keys, [int(x) for x in dims])), int(h.value)
 
 
 def window_range(overlap: np.ndarray, window_size: int, n_windows: int):

@@ -357,7 +357,7 @@ void probe_numa(hb_ctx* ctx) {
 // A model file as the canonical tensor table (names and forms of herro_b200/weights.py): either the HB200W1 blob, or a
 // TorchScript archive of the same architecture - what the reference's `-m` names (src/inference.rs:185) - read by torchscript.cpp.
 struct ModelFile {
-    uint32_t cfg[10] = {0};  // tokens, emb, reads, stem_k, C, H, layers, F, D, classes
+    uint32_t cfg[13] = {0};  // tokens, emb, reads, stem_k, C, H, layers, F, D, classes, pos_layers, pos_heads, pos_ffn
     std::map<std::string, std::vector<float>> T;
 };
 int read_model_file(const char* path, ModelFile& mf, std::string& err) {
@@ -375,14 +375,16 @@ int read_model_file(const char* path, ModelFile& mf, std::string& err) {
         if (!ts_read_archive(buf.data(), buf.size(), m)) { err = "TorchScript archive: " + m.err; return HB_ERR_MODEL; }
         TsDims d;
         if (!ts_to_canonical(m, 4, d, mf.T, err)) { err = "TorchScript archive: " + err; return HB_ERR_MODEL; }
-        const uint32_t c[10] = {12, 6, 31, (uint32_t)d.stem_k, (uint32_t)d.channels, (uint32_t)d.heads, (uint32_t)d.layers, (uint32_t)d.ffn, (uint32_t)d.collapse, 5};
+        const uint32_t c[13] = {12, 6, 31, (uint32_t)d.stem_k, (uint32_t)d.channels, (uint32_t)d.heads, (uint32_t)d.layers, (uint32_t)d.ffn, (uint32_t)d.collapse, 5,
+                                (uint32_t)d.pos_layers, (uint32_t)d.pos_heads, (uint32_t)d.pos_ffn};
         memcpy(mf.cfg, c, sizeof c);
         return HB_OK;
     }
     if ((size_t)sz < sizeof(BlobHeader)) { err = "model file too small"; return HB_ERR_MODEL; }
     BlobHeader h;
     memcpy(&h, buf.data(), sizeof h);
-    if (memcmp(h.magic, "HB200W1\0", 8) != 0 || h.version != 1) {
+    // VERSION 2 marks a blob with a position-axis stage (header words 10-12), so that a library without it refuses the file
+    if (memcmp(h.magic, "HB200W1\0", 8) != 0 || (h.version != 1 && h.version != 2)) {
         err = "neither an HB200W1 weights blob nor a TorchScript archive";
         return HB_ERR_MODEL;
     }
@@ -422,6 +424,15 @@ int load_weights(hb_ctx* ctx, const char* path) {
     if (wt.layers < 1 || wt.layers > MAX_LAYERS || wt.H < 1 || wt.C % wt.H || (wt.C / wt.H != 16 && wt.C / wt.H != 32) ||
         wt.C % 128 || wt.F % 128 || wt.D % 128 || !(wt.stem_k & 1) || wt.stem_k > 129 || wt.C > 1024)
         return fail(ctx, HB_ERR_MODEL, "unsupported model dimensions (need C,F,D % 128 == 0, head_dim 16 or 32, odd stem_k)");
+    wt.pos_layers = (int)cfg[10]; wt.pos_heads = (int)cfg[11]; wt.pos_ffn = (int)cfg[12];
+    if (wt.pos_layers) {
+        if (wt.pos_layers > MAX_LAYERS)
+            return fail(ctx, HB_ERR_MODEL, "unsupported pos_layers " + std::to_string(wt.pos_layers) + " (at most " + std::to_string(MAX_LAYERS) + ")");
+        if (wt.pos_heads < 1 || wt.D % wt.pos_heads || (wt.D / wt.pos_heads != 32 && wt.D / wt.pos_heads != 64))
+            return fail(ctx, HB_ERR_MODEL, "unsupported pos_heads " + std::to_string(wt.pos_heads) + " (collapse / pos_heads must be 32 or 64)");
+        if (wt.pos_ffn < 128 || wt.pos_ffn % 128)
+            return fail(ctx, HB_ERR_MODEL, "unsupported pos_ffn " + std::to_string(wt.pos_ffn) + " (must be a positive multiple of 128)");
+    }
     std::unordered_map<std::string, std::pair<const float*, size_t>> T;
     for (auto& kv : mf.T) T[kv.first] = {kv.second.data(), kv.second.size()};
     auto need = [&](const std::string& n, size_t count, const float*& hostp) -> bool {
@@ -469,6 +480,17 @@ int load_weights(hb_ctx* ctx, const char* path) {
     ok = ok && get("lnf_g", C, wt.lnf_g) && get("lnf_b", C, wt.lnf_b) && get("wc", (size_t)D * 31 * C, wt.wc) &&
          get("bc", D, wt.bc) && get("wb", 5 * (size_t)D, wt.wb) && get("bb", 5, wt.bb) && get("wi", D, wt.wi) &&
          get("bi", 1, wt.bi);
+    const size_t P = (size_t)wt.pos_ffn;
+    std::vector<const float*> pos_w(4 * (size_t)wt.pos_layers);  // wqkv, wo, w1, w2 of each position layer (device, fp32)
+    for (int l = 0; ok && l < wt.pos_layers; l++) {
+        const std::string p = "p" + std::to_string(l) + ".";
+        PosLayer& ly = wt.pos[l];
+        const float** w4 = &pos_w[4 * (size_t)l];
+        ok = get(p + "ln1_g", D, ly.ln1_g) && get(p + "ln1_b", D, ly.ln1_b) && get(p + "wqkv", (size_t)3 * D * D, w4[0]) &&
+             get(p + "bqkv", 3 * (size_t)D, ly.bqkv) && get(p + "wo", (size_t)D * D, w4[1]) && get(p + "bo", D, ly.bo) &&
+             get(p + "ln2_g", D, ly.ln2_g) && get(p + "ln2_b", D, ly.ln2_b) && get(p + "w1", P * D, w4[2]) &&
+             get(p + "b1", P, ly.b1) && get(p + "w2", (size_t)D * P, w4[3]) && get(p + "b2", D, ly.b2);
+    }
     if (!ok) return ctx->err.rfind("cuda", 0) == 0 ? HB_ERR_CUDA : HB_ERR_MODEL;
     // bf16 hi/lo split of the contraction weights for the wgmma path (gemm_tc.cu)
     if (cudaDeviceGetAttribute(&wt.num_sms, cudaDevAttrMultiProcessorCount, ctx->device) != cudaSuccess) wt.num_sms = 132;
@@ -486,6 +508,12 @@ int load_weights(hb_ctx* ctx, const char* path) {
             !split(ly.w1, (size_t)F * C, ly.s_1) || !split(ly.w2, (size_t)C * F, ly.s_2)) return HB_ERR_CUDA;
     }
     if (!split(wt.wc, (size_t)D * 31 * C, wt.s_c)) return HB_ERR_CUDA;
+    for (int l = 0; l < wt.pos_layers; l++) {
+        PosLayer& ly = wt.pos[l];
+        const float* const* w4 = &pos_w[4 * (size_t)l];
+        if (!split(w4[0], (size_t)3 * D * D, ly.s_qkv) || !split(w4[1], (size_t)D * D, ly.s_o) || !split(w4[2], P * D, ly.s_1) ||
+            !split(w4[3], (size_t)D * P, ly.s_2)) return HB_ERR_CUDA;
+    }
     // head-grouped copy of Wqkv / bqkv for the fused QKV+attention kernel: row (h, s, d) = row s*C + h*32 + d (s = q,k,v)
     if (C == 128 && wt.H == 4) {
         for (int l = 0; l < wt.layers; l++) {
@@ -602,15 +630,16 @@ size_t carve_rows(BatchView& b, uint8_t* base) {
 }
 
 // Forward region, sized from the supported positions once the first wait has counted them: the work list, the logits and
-// the workspace of one forward pass
-size_t carve_fwd(const hb_ctx* ctx, BatchView& b, FwdBufs& f, uint64_t n_sup, uint8_t* base) {
+// the workspace of one forward pass.  A pass holds whole windows (launch_tail), so it is sized for chunk_pos positions or
+// the largest window, whichever is larger.
+size_t carve_fwd(const hb_ctx* ctx, BatchView& b, FwdBufs& f, uint64_t n_sup, uint32_t max_nsup, uint8_t* base) {
     const size_t n = std::max<uint64_t>(n_sup, 1);
     Carve c{base};
     c(b.fwd_win, n);
     c(b.fwd_row, n);
     c(f.logits, n * 5);
     c(f.info, n);
-    c(f.ws, fwd_workspace_bytes(ctx->wt, (uint32_t)std::min<uint64_t>(ctx->chunk_pos, n)));
+    c(f.ws, fwd_workspace_bytes(ctx->wt, (uint32_t)std::min<uint64_t>(std::max(ctx->chunk_pos, max_nsup), n)));
     return c.bytes;
 }
 
@@ -668,12 +697,19 @@ int zero_scratch(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b) {
     return HB_OK;
 }
 
-// The forward + consensus part once the number of supported positions is known.
-int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, uint64_t n_sup, uint64_t* launches) {
+// The forward + consensus part once the supported positions of every window (nsup[nw]) are known.  A forward pass takes
+// as many whole windows as fit in chunk_pos positions; a window larger than that is a pass of its own.
+int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, const uint32_t* nsup, size_t nw, uint64_t* launches) {
     *launches += launch_features_c2(b, L->stream, L->kt);
-    for (uint64_t n0 = 0; n0 < n_sup; n0 += ctx->chunk_pos) {
-        const uint32_t np = (uint32_t)std::min<uint64_t>(ctx->chunk_pos, n_sup - n0);
-        *launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, np, f.ws, f.logits, f.info, L->stream, L->kt);
+    uint64_t n0 = 0;
+    for (size_t w0 = 0; w0 < nw;) {
+        uint64_t np = nsup[w0];
+        size_t w1 = w0 + 1;
+        while (w1 < nw && np + nsup[w1] <= ctx->chunk_pos) np += nsup[w1++];
+        if (np) *launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, (uint32_t)np, (uint32_t)w0, (uint32_t)(w1 - w0), f.ws, f.logits,
+                                                  f.info, L->stream, L->kt);
+        n0 += np;
+        w0 = w1;
     }
     CK(cudaEventRecord(L->ev[4], L->stream));
     *launches += launch_consensus(b, L->stream, L->kt);
@@ -732,6 +768,7 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         CK(cudaEventRecord(L->ev[2], L->stream));
         launches += launch_features_c1(b, L->stream, L->kt);  // ref_lmax + scan; the work list needs its buffers first
         CK(cudaMemcpyAsync(h.cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaMemcpyAsync(h.nsup, b.w_nsup, nw * 4, cudaMemcpyDeviceToHost, L->stream));  // the forward passes end at window boundaries
         PHASE(1);
         SYNC_TIMED();
         PHASE(2);
@@ -742,11 +779,12 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         if (rc) return rc;
     }
     const uint64_t n_sup = (uint64_t)h.cnt[CNT_NSUP] | ((uint64_t)h.cnt[CNT_NSUP + 1] << 32);
+    const uint32_t max_nsup = nw ? *std::max_element(h.nsup, h.nsup + nw) : 0;
     FwdBufs f;
-    CK(L->d_fwd.grow(carve_fwd(ctx, b, f, n_sup, nullptr)));
-    carve_fwd(ctx, b, f, n_sup, L->d_fwd.as<uint8_t>());
+    CK(L->d_fwd.grow(carve_fwd(ctx, b, f, n_sup, max_nsup, nullptr)));
+    carve_fwd(ctx, b, f, n_sup, max_nsup, L->d_fwd.as<uint8_t>());
     CK(cudaEventRecord(L->ev[3], L->stream));
-    rc = launch_tail(ctx, L, b, f, n_sup, &launches);
+    rc = launch_tail(ctx, L, b, f, h.nsup, nw, &launches);
     if (rc) return rc;
 
     // ---- D2H: per-window metadata, then exactly the emitted bytes
@@ -754,7 +792,6 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     CK(cudaMemcpyAsync(h.outlen, b.w_outlen, nw * 4, cudaMemcpyDeviceToHost, L->stream));
     CK(cudaMemcpyAsync(h.nsel, b.w_nsel, nw * 4, cudaMemcpyDeviceToHost, L->stream));
     CK(cudaMemcpyAsync(h.L, b.w_L, nw * 4, cudaMemcpyDeviceToHost, L->stream));
-    CK(cudaMemcpyAsync(h.nsup, b.w_nsup, nw * 4, cudaMemcpyDeviceToHost, L->stream));
     CK(cudaMemcpyAsync(h.terr, b.tgt_err, nt * 4, cudaMemcpyDeviceToHost, L->stream));
     CK(cudaMemcpyAsync(h.sel, b.sel_ow, nw * TOP_K * 4, cudaMemcpyDeviceToHost, L->stream));
     // the emitted bytes of all windows are contiguous from offset 0 and number at most one per matrix row, so the
@@ -783,6 +820,9 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         uint64_t cf[16];
         forward_class_flops_per_pos(ctx->wt, cf);
         for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) S.class_flops[i] += cf[i] * n_sup;
+        const uint64_t pa = pos_attn_flops(ctx->wt, h.nsup, nw);
+        S.class_flops[K_POS_ATTN] += pa;
+        S.forward_flops += pa;
     }
 
     // ---- per-read reassembly (src/consensus.rs:90-111,222-226)
@@ -1001,7 +1041,8 @@ void presize_lane(hb_ctx* ctx, hb_ctx::Lane* L, const hb_ctx::LaneSizes& T) {
     if (ll.valid) {  // the regions moved with their contents: carving the kept view's counts again gives the same offsets
         carve_batch(ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, L->d_batch.as<uint8_t>());
         carve_rows(ll.view, L->d_rows.as<uint8_t>());
-        carve_fwd(ctx, ll.view, ll.fwd, ll.n_sup, L->d_fwd.as<uint8_t>());
+        const uint32_t max_nsup = ll.w_nsup.empty() ? 0 : *std::max_element(ll.w_nsup.begin(), ll.w_nsup.end());
+        carve_fwd(ctx, ll.view, ll.fwd, ll.n_sup, max_nsup, L->d_fwd.as<uint8_t>());
     }
 }
 
@@ -1221,6 +1262,14 @@ extern "C" {
 
 int hb_inspect_model(const char* model_path, uint32_t dims[6], uint64_t* params_hash, char* err, size_t err_cap) {
     if (!model_path || !dims) return HB_ERR_ARG;
+    uint32_t d9[9];
+    const int rc = hb_inspect_model_ex(model_path, d9, params_hash, err, err_cap);
+    if (rc == HB_OK) memcpy(dims, d9, 6 * sizeof(uint32_t));
+    return rc;
+}
+
+int hb_inspect_model_ex(const char* model_path, uint32_t dims[9], uint64_t* params_hash, char* err, size_t err_cap) {
+    if (!model_path || !dims) return HB_ERR_ARG;
     ModelFile mf;
     std::string e;
     const int rc = read_model_file(model_path, mf, e);
@@ -1229,6 +1278,7 @@ int hb_inspect_model(const char* model_path, uint32_t dims[6], uint64_t* params_
         return rc;
     }
     for (int i = 0; i < 6; i++) dims[i] = mf.cfg[3 + i];
+    for (int i = 0; i < 3; i++) dims[6 + i] = mf.cfg[10 + i];
     if (params_hash) {  // FNV-1a over the canonical tensors in name order: equal for a blob and an archive of the same weights
         uint64_t h = 1469598103934665603ull;
         for (auto& kv : mf.T) {
@@ -1818,6 +1868,59 @@ int hb_selftest_gemm(int cuda_device, uint32_t M, uint32_t N, uint32_t K, int ac
     return rc;
 }
 
+int hb_selftest_pos_attention(int cuda_device, const uint32_t* lens, uint32_t n_seq, uint32_t heads, uint32_t head_dim,
+                              const float* qkv, float* out, float* ms) {
+    if (!lens || !qkv || !out || heads == 0 || (head_dim != 32 && head_dim != 64)) return HB_ERR_ARG;
+    if (cudaSetDevice(cuda_device) != cudaSuccess) return HB_ERR_CUDA;
+    const size_t D = (size_t)heads * head_dim;
+    std::vector<uint64_t> base(n_seq);
+    uint64_t rows = 0;
+    for (uint32_t i = 0; i < n_seq; i++) { base[i] = rows; rows += lens[i]; }
+    const size_t r1 = std::max<uint64_t>(rows, 1), s1 = std::max<uint32_t>(n_seq, 1);
+    float* dq = nullptr;
+    uint64_t* db = nullptr;
+    uint32_t* dl = nullptr;
+    __nv_bfloat16 *ohi = nullptr, *olo = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    cudaError_t e = cudaMalloc(&dq, r1 * 3 * D * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&db, s1 * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&dl, s1 * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&ohi, r1 * D * 2);
+    if (e == cudaSuccess) e = cudaMalloc(&olo, r1 * D * 2);
+    if (e == cudaSuccess) e = cudaMemcpy(dq, qkv, rows * 3 * D * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_seq) e = cudaMemcpy(db, base.data(), n_seq * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_seq) e = cudaMemcpy(dl, lens, n_seq * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(ohi, 0, r1 * D * 2);
+    if (e == cudaSuccess) e = cudaMemset(olo, 0, r1 * D * 2);
+    if (e == cudaSuccess) {
+        cudaEventCreate(&e0);
+        cudaEventCreate(&e1);
+        // the launcher of the forward's position-axis stage (forward.cu), on one chunk holding every sequence
+        const PosAttnArgs pa{dq, 3 * D, db, dl, 0, n_seq, (int)D, (int)heads, ohi, olo, D};
+        cudaEventRecord(e0);
+        e = pos_attention(pa, 0);
+        cudaEventRecord(e1);
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    }
+    if (e == cudaSuccess) {
+        std::vector<uint16_t> h1(rows * D), h2(rows * D);
+        e = cudaMemcpy(h1.data(), ohi, h1.size() * 2, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(h2.data(), olo, h2.size() * 2, cudaMemcpyDeviceToHost);
+        for (size_t i = 0; e == cudaSuccess && i < h1.size(); i++) {
+            const uint32_t a = (uint32_t)h1[i] << 16, b2 = (uint32_t)h2[i] << 16;
+            float fa, fb;
+            memcpy(&fa, &a, 4); memcpy(&fb, &b2, 4);
+            out[i] = fa + fb;
+        }
+        if (e == cudaSuccess && ms) cudaEventElapsedTime(ms, e0, e1);
+    }
+    if (e != cudaSuccess) g_create_err = std::string("selftest: ") + cudaGetErrorString(e);
+    cudaFree(dq); cudaFree(db); cudaFree(dl); cudaFree(ohi); cudaFree(olo);
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+    return e == cudaSuccess ? HB_OK : HB_ERR_CUDA;
+}
+
 int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
     if (!ctx || !ms) return HB_ERR_ARG;
     std::unique_lock<std::mutex> lk(ctx->mu);
@@ -1837,7 +1940,7 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
         launches += launch_features_a(b, L->stream, L->kt);
         launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
         launches += launch_features_c1(b, L->stream, L->kt);
-        rc = launch_tail(ctx, L, b, L->last.fwd, L->last.n_sup, &launches);
+        rc = launch_tail(ctx, L, b, L->last.fwd, L->last.w_nsup.data(), L->last.w_nsup.size(), &launches);
         if (rc) return rc;
     }
     CK(cudaEventRecord(L->ev[7], L->stream));

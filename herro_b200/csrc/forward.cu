@@ -321,6 +321,9 @@ __global__ void k_heads(BatchView b, FwdWeights wt, uint32_t n0, uint32_t npos, 
 struct FwdWs {
     float *X, *QKV, *Z;
     __nv_bfloat16 *Hhi, *Hlo, *Fhi, *Flo;
+    // position-axis stage (only carved when the model has one): its QKV, LayerNorm / attention output and hidden layer
+    float* Pqkv = nullptr;
+    __nv_bfloat16 *Phi = nullptr, *Plo = nullptr, *PFhi = nullptr, *PFlo = nullptr;
     size_t bytes;
 };
 static bool ffn_is_fused(const FwdWeights& wt) { return wt.C == 128 && wt.F == 512 && !wt.no_fuse_ln && !wt.no_fuse_ffn; }
@@ -340,6 +343,13 @@ static FwdWs carve(const FwdWeights& wt, size_t npos, uint8_t* base) {
     const size_t TF = ffn_is_fused(wt) ? 0 : T;
     w.Fhi = (__nv_bfloat16*)(base + o); o += al256(TF * wt.F * 2);
     w.Flo = (__nv_bfloat16*)(base + o); o += al256(TF * wt.F * 2);
+    if (wt.pos_layers) {
+        w.Pqkv = (float*)(base + o); o += al256(np * 3 * wt.D * 4);
+        w.Phi = (__nv_bfloat16*)(base + o); o += al256(np * wt.D * 2);
+        w.Plo = (__nv_bfloat16*)(base + o); o += al256(np * wt.D * 2);
+        w.PFhi = (__nv_bfloat16*)(base + o); o += al256(np * wt.pos_ffn * 2);
+        w.PFlo = (__nv_bfloat16*)(base + o); o += al256(np * wt.pos_ffn * 2);
+    }
     w.bytes = o;
     return w;
 }
@@ -383,6 +393,17 @@ static void gemm_ln(const FwdWeights& wt, const __nv_bfloat16* Ahi, const __nv_b
     kt.end();
 }
 
+// contractions of the position-axis stage per supported position: QKV, out-projection, FFN1, FFN2
+static uint64_t pos_gemm_flops_per_pos(const FwdWeights& wt) {
+    const uint64_t D = wt.D, P = wt.pos_ffn;
+    return (uint64_t)wt.pos_layers * 2 * (D * 3 * D + D * D + 2 * D * P);
+}
+uint64_t pos_attn_flops(const FwdWeights& wt, const uint32_t* nsup, size_t nwin) {
+    uint64_t s2 = 0;
+    for (size_t w = 0; w < nwin; w++) s2 += (uint64_t)nsup[w] * nsup[w];
+    return 4 * (uint64_t)wt.D * wt.pos_layers * s2;  // per layer and head: QK^T and PV, 2 * n^2 * head_dim each
+}
+
 // algorithmic FLOPs per supported position (2 * MACs), and the part that is dense contractions
 uint64_t forward_flops_per_pos(const FwdWeights& wt, uint64_t* gemm_flops) {
     const uint64_t C = wt.C, F = wt.F, D = wt.D, K = wt.stem_k, S = R_COLS, dh = wt.C / wt.H;
@@ -391,7 +412,7 @@ uint64_t forward_flops_per_pos(const FwdWeights& wt, uint64_t* gemm_flops) {
     const uint64_t per_layer_attn = (uint64_t)wt.H * 2 * 2 * S * S * dh;
     const uint64_t collapse = 2 * S * C * D;
     const uint64_t heads = 2 * D * 6;
-    const uint64_t g = (uint64_t)wt.layers * per_layer_gemm + collapse;
+    const uint64_t g = (uint64_t)wt.layers * per_layer_gemm + collapse + pos_gemm_flops_per_pos(wt);
     if (gemm_flops) *gemm_flops = g;
     return stem + g + (uint64_t)wt.layers * per_layer_attn + heads;
 }
@@ -407,12 +428,44 @@ void forward_class_flops_per_pos(const FwdWeights& wt, uint64_t (&out)[16]) {
     out[K_GEMM] += 2 * S * C * D;
     if (oproj_in_ffn(wt)) out[K_FFN] += L * oproj; else out[K_GEMM] += L * oproj;
     if (ffn_is_fused(wt)) out[K_FFN] += L * ffn; else out[K_GEMM] += L * ffn;
+    out[K_GEMM] += pos_gemm_flops_per_pos(wt);
     out[K_HEADS] = 2 * D * 6;
 }
 
-// Runs positions [n0, n0+npos) of the work list.  Returns the number of kernel launches.
-int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, uint32_t npos, uint8_t* wsb,
-                         float* logits, float* info, cudaStream_t st, KTimer& kt) {
+// The position-axis encoder stage on Z [np_pad][D] (the collapse output), in place: Z += pe, then per layer
+// Z += Wo·Attn(LN1(Z)) and Z += W2·relu(W1·LN2(Z)).  The chunk holds whole windows [w0, w0+nwin); each is one sequence.
+static int pos_stage(const BatchView& b, const FwdWeights& wt, const FwdWs& ws, uint32_t n0, uint32_t npos, uint32_t w0,
+                     uint32_t nwin, size_t np_pad, cudaStream_t st, KTimer& kt) {
+    const int D = wt.D, P = wt.pos_ffn;
+    const unsigned ln_blocks = (unsigned)((np_pad * 32 + 255) / 256);
+    int nl = 0;
+    kt.begin(K_LAYERNORM);
+    launch_pos_embed(b, n0, npos, D, ws.Z, st);
+    k_layernorm<<<ln_blocks, 256, 0, st>>>(ws.Z, ws.Phi, ws.Plo, wt.pos[0].ln1_g, wt.pos[0].ln1_b, (uint32_t)np_pad, D);
+    kt.end(); nl += 2;
+    for (int l = 0; l < wt.pos_layers; l++) {
+        const PosLayer& ly = wt.pos[l];
+        gemm(wt, GEMM_OUT_F32, ws.Phi, ws.Plo, D, ly.s_qkv, ly.bqkv, ws.Pqkv, nullptr, 3 * D, nullptr, nullptr, 0, np_pad, 3 * D, D, st, kt); nl++;
+        // the attention output goes over the LN buffers, which the QKV contraction has consumed (stream order); the rows of
+        // the last tile's pad positions are in no window and keep their finite LayerNorm values
+        PosAttnArgs pa{ws.Pqkv, (size_t)3 * D, b.w_supbase + w0, b.w_nsup + w0, n0, nwin, D, wt.pos_heads, ws.Phi, ws.Plo, (size_t)D};
+        kt.begin(K_POS_ATTN); pos_attention(pa, st); kt.end(); nl++;
+        gemm(wt, GEMM_OUT_F32_RES, ws.Phi, ws.Plo, D, ly.s_o, ly.bo, ws.Z, ws.Z, D, nullptr, nullptr, 0, np_pad, D, D, st, kt); nl++;
+        kt.begin(K_LAYERNORM); k_layernorm<<<ln_blocks, 256, 0, st>>>(ws.Z, ws.Phi, ws.Plo, ly.ln2_g, ly.ln2_b, (uint32_t)np_pad, D); kt.end(); nl++;
+        gemm(wt, GEMM_OUT_SPLIT_RELU, ws.Phi, ws.Plo, D, ly.s_1, ly.b1, nullptr, nullptr, 0, ws.PFhi, ws.PFlo, P, np_pad, P, D, st, kt); nl++;
+        gemm(wt, GEMM_OUT_F32_RES, ws.PFhi, ws.PFlo, P, ly.s_2, ly.b2, ws.Z, ws.Z, D, nullptr, nullptr, 0, np_pad, D, P, st, kt); nl++;
+        if (l + 1 < wt.pos_layers) {
+            kt.begin(K_LAYERNORM);
+            k_layernorm<<<ln_blocks, 256, 0, st>>>(ws.Z, ws.Phi, ws.Plo, wt.pos[l + 1].ln1_g, wt.pos[l + 1].ln1_b, (uint32_t)np_pad, D);
+            kt.end(); nl++;
+        }
+    }
+    return nl;
+}
+
+// Runs positions [n0, n0+npos) of the work list, the whole windows [w0, w0+nwin).  Returns the number of kernel launches.
+int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, uint32_t npos, uint32_t w0, uint32_t nwin,
+                         uint8_t* wsb, float* logits, float* info, cudaStream_t st, KTimer& kt) {
     const int C = wt.C, F = wt.F, D = wt.D, H = wt.H;
     const size_t np_pad = (size_t)(npos + 127) / 128 * 128;
     const size_t T = np_pad * TOK_PER_POS;
@@ -501,6 +554,7 @@ int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, 
     // read-axis collapse: row n = the 31*C contiguous values of position n (token 31 excluded)
     gemm(wt, GEMM_OUT_F32_RELU, ws.Hhi, ws.Hlo, (size_t)TOK_PER_POS * C, wt.s_c, wt.bc, ws.Z, nullptr, D, nullptr, nullptr, 0, np_pad, D,
          R_COLS * C, st, kt); nl++;
+    if (wt.pos_layers) nl += pos_stage(b, wt, ws, n0, npos, w0, nwin, np_pad, st, kt);
     kt.begin(K_HEADS);
     k_heads<<<(unsigned)(((size_t)npos * 32 + 127) / 128), 128, 0, st>>>(b, wt, n0, npos, ws.Z, logits, info);
     kt.end(); nl++;

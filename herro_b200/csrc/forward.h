@@ -22,6 +22,11 @@ struct FwdLayer {
     const float* bqkvp = nullptr;  // bqkv in the same order; nullptr: fused kernel unavailable
 };
 
+struct PosLayer {  // an encoder layer of the position-axis stage (width D, pos_heads heads, pos_ffn hidden)
+    const float *ln1_g, *ln1_b, *bqkv, *bo, *ln2_g, *ln2_b, *b1, *b2;
+    SplitW s_qkv, s_o, s_1, s_2;
+};
+
 struct FwdWeights {
     int stem_k, C, H, layers, F, D;
     const float* stem_tab;  // [K][12][C]  = sum_e stem_w[c][e][j] * emb[t][e]   (embedding folded into the conv)
@@ -36,6 +41,9 @@ struct FwdWeights {
     int num_sms;
     // debugging aids / A-B parity tests, read from the environment ONCE in hb_create (HERRO_B200_NO_FUSE_{LN,FFN,ATTN})
     int no_fuse_ln = 0, no_fuse_ffn = 0, no_fuse_attn = 0, no_fuse_oproj = 0;
+    // position-axis encoder stage after the collapse (0 layers: none); kept last so the fields above keep their offsets
+    int pos_layers = 0, pos_heads = 0, pos_ffn = 0;
+    PosLayer pos[MAX_LAYERS];
 };
 
 // gemm_tc.cu
@@ -91,6 +99,23 @@ struct StemArgs {  // k_stem_tc: the stem as a contraction over taps x 16 featur
     __nv_bfloat16 *out_hi = nullptr, *out_lo = nullptr;    // [positions*32][128]; nullptr: X only
 };
 cudaError_t stem_tc(const BatchView& b, const StemArgs& a, int num_sms, cudaStream_t st);
+// pos_attn.cu: attention over variable-length sequences of rows (sequence i = rows [seq_base[i] - base_sub, + seq_len[i])
+// of `qkv`, whose row holds q | k | v, D each, heads of D / heads in {32, 64}); keys past a sequence's length are masked.
+// Writes the attention output of each sequence row as split bf16; rows outside every sequence are not written.
+struct PosAttnArgs {
+    const float* qkv;                // [rows][ld_qkv] fp32
+    size_t ld_qkv;
+    const uint64_t* seq_base;        // [n_seq]
+    const uint32_t* seq_len;         // [n_seq]
+    uint64_t base_sub;
+    uint32_t n_seq;
+    int D, heads;
+    __nv_bfloat16 *out_hi, *out_lo;  // [rows][ldo]
+    size_t ldo;
+};
+cudaError_t pos_attention(const PosAttnArgs& a, cudaStream_t st);
+// Z[n] += sinusoidal encoding of the index of position n0 + n within its window, n < npos (Z: [npos][D] fp32)
+void launch_pos_embed(const BatchView& b, uint32_t n0, uint32_t npos, int D, float* Z, cudaStream_t st);
 cudaError_t split_weights(const float* w, size_t n, void** hi, void** lo);
 cudaError_t gemm_tc(const GemmArgs& a, int num_sms, cudaStream_t st);
 // forward.cu (fp32 SIMT contraction: the self test's reference)
@@ -132,15 +157,18 @@ struct KTimer {
     void destroy() { for (auto e : pool) cudaEventDestroy(e); pool.clear(); }
 };
 enum { K_TOKENIZE = 0, K_PASS1, K_SCORES, K_PASS2A, K_SCAN, K_PILEUP, K_LISTS, K_STEM, K_LAYERNORM, K_GEMM, K_ATTENTION,
-       K_HEADS, K_CONSENSUS, K_FFN, K_QKV_ATTN };
+       K_HEADS, K_CONSENSUS, K_FFN, K_QKV_ATTN, K_POS_ATTN };
 
 // Scratch is carved from one allocation into arrays that each start 256-byte aligned, the alignment a separate cudaMalloc
 // would give: TMA operands and 16-byte row stores rely on it.
 inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 size_t fwd_workspace_bytes(const FwdWeights& wt, uint32_t chunk_pos);
-int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, uint32_t npos, uint8_t* ws,
-                         float* logits, float* info, cudaStream_t st, KTimer& kt);
+// Runs positions [n0, n0+npos) of the work list: whole windows [w0, w0+nwin) (the position-axis stage attends within them)
+int launch_forward_chunk(const BatchView& b, const FwdWeights& wt, uint32_t n0, uint32_t npos, uint32_t w0, uint32_t nwin,
+                         uint8_t* ws, float* logits, float* info, cudaStream_t st, KTimer& kt);
 uint64_t forward_flops_per_pos(const FwdWeights& wt, uint64_t* gemm_flops);
+// FLOPs of the position-axis attention (QK^T and PV) of windows with the given supported-position counts
+uint64_t pos_attn_flops(const FwdWeights& wt, const uint32_t* nsup, size_t nwin);
 // algorithmic FLOPs per supported position attributed to the kernel class that executes them on the active code path
 void forward_class_flops_per_pos(const FwdWeights& wt, uint64_t (&out)[16]);
 

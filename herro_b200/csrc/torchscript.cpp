@@ -410,8 +410,28 @@ bool ts_to_canonical(const TsModel& m, int heads_hint, TsDims& d, std::map<std::
             !put(q + "b1", p + "ff1.bias", 1, F) || !put(q + "w2", p + "ff2.weight", 2, Cs * F) || !put(q + "b2", p + "ff2.bias", 1, Cs))
             return false;
     }
-    return put("lnf_g", "lnf.weight", 1, Cs) && put("lnf_b", "lnf.bias", 1, Cs) && put("wc", "collapse.weight", 2, D * 31 * Cs) && put("bc", "collapse.bias", 1, D) &&
-           put("wb", "base_head.weight", 2, 5 * D) && put("bb", "base_head.bias", 1, 5) && put("wi", "info_head.weight", 2, D) && put("bi", "info_head.bias", 1, 1);
+    if (!(put("lnf_g", "lnf.weight", 1, Cs) && put("lnf_b", "lnf.bias", 1, Cs) && put("wc", "collapse.weight", 2, D * 31 * Cs) && put("bc", "collapse.bias", 1, D) &&
+          put("wb", "base_head.weight", 2, 5 * D) && put("bb", "base_head.bias", 1, 5) && put("wi", "info_head.weight", 2, D) && put("bi", "info_head.bias", 1, 1)))
+        return false;
+    // optional encoder stage across each window's supported positions (width D): pos_layers.{l}.*, head count pos_layers.0.H
+    int pl = 0;
+    while (get("pos_layers." + std::to_string(pl) + ".qkv.weight")) pl++;
+    if (pl == 0) return true;
+    auto ph = m.ints.find("pos_layers.0.H");
+    if (ph == m.ints.end()) { err = "the archive has position layers but no head count 'pos_layers.0.H'"; return false; }
+    const TsTensor* pf1 = need("pos_layers.0.ff1.weight", 2);
+    if (!pf1) return false;
+    d.pos_layers = pl; d.pos_heads = (int)ph->second; d.pos_ffn = (int)pf1->shape[0];
+    const size_t P = (size_t)d.pos_ffn;
+    for (int l = 0; l < pl; l++) {
+        const std::string p = "pos_layers." + std::to_string(l) + ".", q = "p" + std::to_string(l) + ".";
+        if (!put(q + "ln1_g", p + "ln1.weight", 1, D) || !put(q + "ln1_b", p + "ln1.bias", 1, D) || !put(q + "wqkv", p + "qkv.weight", 2, 3 * D * D) ||
+            !put(q + "bqkv", p + "qkv.bias", 1, 3 * D) || !put(q + "wo", p + "out.weight", 2, D * D) || !put(q + "bo", p + "out.bias", 1, D) ||
+            !put(q + "ln2_g", p + "ln2.weight", 1, D) || !put(q + "ln2_b", p + "ln2.bias", 1, D) || !put(q + "w1", p + "ff1.weight", 2, P * D) ||
+            !put(q + "b1", p + "ff1.bias", 1, P) || !put(q + "w2", p + "ff2.weight", 2, D * P) || !put(q + "b2", p + "ff2.bias", 1, D))
+            return false;
+    }
+    return true;
 }
 
 }  // namespace hb

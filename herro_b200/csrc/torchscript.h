@@ -14,7 +14,7 @@ struct TsModel {
     std::map<std::string, int64_t> ints;       // integer attributes of the module tree ("layers.0.H")
     std::string err;
 };
-struct TsDims { int stem_k = 0, channels = 0, heads = 0, layers = 0, ffn = 0, collapse = 0; };
+struct TsDims { int stem_k = 0, channels = 0, heads = 0, layers = 0, ffn = 0, collapse = 0, pos_layers = 0, pos_heads = 0, pos_ffn = 0; };
 
 bool ts_is_zip(const uint8_t* buf, size_t n);
 bool ts_read_archive(const uint8_t* buf, size_t n, TsModel& out);

@@ -22,7 +22,8 @@ from dataclasses import dataclass, asdict
 import numpy as np
 
 MAGIC = b"HB200W1\0"
-VERSION = 1
+VERSION = 1         # a blob with position layers is VERSION_POS, so that a library without the stage rejects it
+VERSION_POS = 2
 N_READS = 31        # TOP_K_SORT + 1, src/features.rs:22
 N_TOKENS = 12       # BASES_MAP alphabet + padding, src/inference.rs:15,23-31
 EMB_DIM = 6         # as in the only shipped graph (resources/model.pt: Embedding(12, 6, padding_idx=11))
@@ -37,6 +38,9 @@ class NetConfig:
     layers: int = 2
     ffn: int = 512
     collapse: int = 256     # read-axis collapse (legacy: Conv2d(128->256, k=(1,31)))
+    pos_layers: int = 0     # encoder layers across each window's supported positions (0: no such stage)
+    pos_heads: int = 0
+    pos_ffn: int = 0
 
     @property
     def head_dim(self):
@@ -67,6 +71,17 @@ def tensor_shapes(cfg: NetConfig):
         "wb": (N_CLASSES, D), "bb": (N_CLASSES,),
         "wi": (1, D), "bi": (1,),
     })
+    P = cfg.pos_ffn
+    for l in range(cfg.pos_layers):  # after "bi": the random draws of every other tensor stay those of the graph without the stage
+        p = f"p{l}."
+        shapes.update({
+            p + "ln1_g": (D,), p + "ln1_b": (D,),
+            p + "wqkv": (3 * D, D), p + "bqkv": (3 * D,),
+            p + "wo": (D, D), p + "bo": (D,),
+            p + "ln2_g": (D,), p + "ln2_b": (D,),
+            p + "w1": (P, D), p + "b1": (P,),
+            p + "w2": (D, P), p + "b2": (D,),
+        })
     return shapes
 
 
@@ -107,7 +122,7 @@ def save_blob(path: str, cfg: NetConfig, tensors: dict) -> None:
         if tuple(tensors[n].shape) != tuple(shapes[n]):
             raise ValueError(f"{n}: shape {tensors[n].shape} != {shapes[n]}")
     cfgv = [N_TOKENS, EMB_DIM, N_READS, cfg.stem_k, cfg.channels, cfg.heads, cfg.layers, cfg.ffn, cfg.collapse,
-            N_CLASSES] + [0] * 6
+            N_CLASSES, cfg.pos_layers, cfg.pos_heads, cfg.pos_ffn] + [0] * 3
     off = _HDR.size + _ENT.size * len(names)
     off = (off + 63) // 64 * 64
     ents, blobs = [], []
@@ -118,7 +133,7 @@ def save_blob(path: str, cfg: NetConfig, tensors: dict) -> None:
         blobs.append((off, a.tobytes()))
         off = (off + a.nbytes + 63) // 64 * 64
     with open(path, "wb") as f:
-        f.write(_HDR.pack(MAGIC, VERSION, len(names), *cfgv))
+        f.write(_HDR.pack(MAGIC, VERSION_POS if cfg.pos_layers else VERSION, len(names), *cfgv))
         for e in ents:
             f.write(e)
         for o, b in blobs:
@@ -131,11 +146,12 @@ def load_blob(path: str):
     with open(path, "rb") as f:
         buf = f.read()
     magic, ver, nt, *cfgv = _HDR.unpack_from(buf, 0)
-    if magic != MAGIC or ver != VERSION:
+    if magic != MAGIC or ver not in (VERSION, VERSION_POS):
         raise ValueError("not an HB200W1 weights blob")
     if cfgv[0] != N_TOKENS or cfgv[1] != EMB_DIM or cfgv[2] != N_READS or cfgv[9] != N_CLASSES:
         raise ValueError("unsupported fixed dimensions in weights blob")
-    cfg = NetConfig(stem_k=cfgv[3], channels=cfgv[4], heads=cfgv[5], layers=cfgv[6], ffn=cfgv[7], collapse=cfgv[8])
+    cfg = NetConfig(stem_k=cfgv[3], channels=cfgv[4], heads=cfgv[5], layers=cfgv[6], ffn=cfgv[7], collapse=cfgv[8],
+                    pos_layers=cfgv[10], pos_heads=cfgv[11], pos_ffn=cfgv[12])
     tensors = {}
     for i in range(nt):
         name, dt, nd, s0, s1, s2, s3, off, nb = _ENT.unpack_from(buf, _HDR.size + i * _ENT.size)

@@ -92,6 +92,9 @@ void hb_destroy(hb_ctx* ctx);
  * layers, ffn, collapse; *params_hash (may be NULL) = FNV-1a-64 over the canonical fp32 tensors in name order, equal for
  * a blob and an archive holding the same weights.  `err` (may be NULL) receives the message on failure. */
 int hb_inspect_model(const char* model_path, uint32_t dims[6], uint64_t* params_hash, char* err, size_t err_cap);
+/* Same, with dims = stem_k, channels, heads, layers, ffn, collapse, pos_layers, pos_heads, pos_ffn: the last three describe
+ * the optional encoder stage across each window's supported positions (all 0 without one). */
+int hb_inspect_model_ex(const char* model_path, uint32_t dims[9], uint64_t* params_hash, char* err, size_t err_cap);
 
 /* Replicate the read store on the GPU.  Layout is HAECRecord verbatim (src/haec_io.rs:19-24,
  * 77-81): seq_words[i] = 2-bit little-endian packing, 32 bases per u64, A0 C1 G2 T3
@@ -168,7 +171,8 @@ int hb_bind_calling_thread(hb_ctx* ctx);
 /* kernel classes of ms_kernel[] / n_kernel[] */
 enum { HB_K_TOKENIZE = 0, HB_K_PASS1, HB_K_SCORES, HB_K_PASS2A, HB_K_SCAN, HB_K_PILEUP, HB_K_LISTS, HB_K_STEM,
        HB_K_LAYERNORM, HB_K_GEMM, HB_K_ATTENTION, HB_K_HEADS, HB_K_CONSENSUS,
-       HB_K_FFN /* fused FFN kernel */, HB_K_QKV_ATTN /* fused QKV projection + attention kernel */ };
+       HB_K_FFN /* fused FFN kernel */, HB_K_QKV_ATTN /* fused QKV projection + attention kernel */,
+       HB_K_POS_ATTN /* attention across a window's supported positions (position-axis stage) */ };
 typedef struct hb_stats {
     uint64_t targets, windows, overlap_windows, rows, supported, corrected_bases;
     uint64_t h2d_bytes, d2h_bytes, kernel_launches, device_launches /* batches */;
@@ -222,6 +226,12 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms);
  * difference, the largest |reference| and both kernel times. */
 int hb_selftest_gemm(int cuda_device, uint32_t M, uint32_t N, uint32_t K, int act, int res, uint32_t lda_extra,
                      float* max_abs_err, float* max_abs_ref, float* ms_tc, float* ms_simt);
+/* Runs the position-axis stage's masked attention kernel, through the launcher the forward uses, on n_seq sequences of
+ * lens[i] rows stored back to back: qkv is [sum lens][3 * heads * head_dim] fp32 (q | k | v), head_dim 32 or 64.  Writes
+ * the attention output [sum lens][heads * head_dim] as the sum of its split bf16 halves, and the kernel's time in *ms
+ * (may be NULL). */
+int hb_selftest_pos_attention(int cuda_device, const uint32_t* lens, uint32_t n_seq, uint32_t heads, uint32_t head_dim,
+                              const float* qkv, float* out, float* ms);
 
 #ifdef __cplusplus
 }
