@@ -533,7 +533,8 @@ int load_weights(hb_ctx* ctx, const char* path) {
             if (!split(dwp, wp.size(), wt.layer[l].s_qkvp)) return HB_ERR_CUDA;
         }
     }
-    // W' of the tensor-core stem: [C][taps*16] = tab (11 token slots), wq twice (q_hi, q_lo columns), zero padding
+    // W' of the tensor-core stem: [C][taps*16] = tab of tokens 0..10, wq twice (q_hi, q_lo columns), tab of the pad token 11
+    // (the batch-padding rows carry it, and a model's emb[11] need not be zero), zero padding
     wt.stem_kblocks = 0;
     if (C == 128 && K <= 64 && !getenv("HERRO_B200_STEM_SIMT")) {
         const int kbl = (K * 16 + 63) / 64, Kp = kbl * 64;
@@ -543,6 +544,7 @@ int load_weights(hb_ctx* ctx, const char* path) {
                 for (int t = 0; t < 11; t++) wp[(size_t)c * Kp + j * 16 + t] = tab[((size_t)j * 12 + t) * C + c];
                 wp[(size_t)c * Kp + j * 16 + 11] = wq[(size_t)j * C + c];
                 wp[(size_t)c * Kp + j * 16 + 12] = wq[(size_t)j * C + c];
+                wp[(size_t)c * Kp + j * 16 + 13] = tab[((size_t)j * 12 + 11) * C + c];
             }
         const float* dwp = nullptr;
         if (!upload(wp.data(), wp.size(), dwp)) return HB_ERR_CUDA;

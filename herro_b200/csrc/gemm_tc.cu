@@ -798,7 +798,8 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_qkv_attn_ws(QkvAttnArgs g, con
 // ------------------------------------------------------------------------------------------------
 // Stem on the tensor cores: Embedding(12,6) ++ qual -> Conv(7->C, k=(K,1)) is linear in the one-hot
 // token and in the quality value, so per read token it is a contraction over K' = taps x 16 features
-// (11 one-hot token slots, q_hi, q_lo, 3 zero) with W'[c][j*16+f] = tab[j][f][c] / wq[j][c].  The A
+// (one-hot token slots 0..10, q_hi, q_lo, a one-hot slot for the pad token 11, 2 zero) with
+// W'[c][j*16+f] = tab[j][f][c] (f < 11), wq[j][c] (f = 11, 12), tab[j][11][c] (f = 13).  The A
 // operand is exact in bf16 (one-hot entries, and the normalised quality carried as two bf16 columns),
 // so two passes (A.W_hi + A.W_lo) reproduce the fp32 result.  Producers synthesise the swizzled A tile
 // straight from the [L',32] token/quality matrix (pad/zero rows of the reference batch as in k_stem).
@@ -862,8 +863,9 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                     tma_load_2d(smem_u32(sA) + BM * 128 + BN * 128, &tmWlo, &full_bar[s], (int)(kb * BK), 0);
                 }
                 // ---- A k-block: 4 taps x 16 features of this row, synthesised arithmetically: bf16 1.0 in the token's one-hot slot
-                //      (features 0..10; '.' has a slot, the pad token 11 and rows outside the reference batch are all zero) and the
-                //      normalised quality as (q_hi, q_lo) in features 11, 12.
+                //      (features 0..10; '.' has a slot), the normalised quality as (q_hi, q_lo) in features 11, 12, and the pad
+                //      token 11 of the reference's batch-padding rows as its own one-hot feature 13.  Rows outside the reference
+                //      batch (0xff) are all zero.
                 uint32_t tk[4], qq[4];
 #pragma unroll
                 for (int tl = 0; tl < 4; tl++) {
@@ -888,6 +890,7 @@ __global__ void __launch_bounds__(S_THREADS, 1) k_stem_tc(BatchView b, StemArgs 
                         const __nv_bfloat16 ql = __float2bfloat16_rn(q - __bfloat162float(qh));
                         w[5] |= (uint32_t)__bfloat16_as_ushort(qh) << 16;  // feature 11 = q_hi
                         w[6] |= (uint32_t)__bfloat16_as_ushort(ql);        // feature 12 = q_lo
+                        if (tok == 11u) w[6] |= 0x3f800000u;               // feature 13 = the pad token's one-hot 1.0
                     }
                     *(uint4*)(sA + (uint32_t)p * 128u + (uint32_t)(((2 * tl) ^ (p & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
                     *(uint4*)(sA + (uint32_t)p * 128u + (uint32_t)(((2 * tl + 1) ^ (p & 7)) << 4)) = make_uint4(w[4], w[5], w[6], w[7]);
