@@ -103,6 +103,7 @@ def load_library():
     fp = C.POINTER(C.c_float)
     L.hb_selftest_gemm.argtypes = [C.c_int, u32, u32, u32, C.c_int, C.c_int, u32, fp, fp, fp, fp]
     L.hb_selftest_pos_attention.argtypes = [C.c_int, u32p, u32, u32, u32, fp, fp, fp]
+    L.hb_forward_batch.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp, vp, u32, vp]
     _lib = L
     return L
 
@@ -110,7 +111,8 @@ def load_library():
 EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "hb_bind_calling_thread", "hb_set_launch_targets", "hb_set_kernel_timing", "hb_extract_windows", "hb_create", "hb_destroy", "hb_upload_reads", "hb_submit_target", "hb_submit_alignments", "hb_flush",
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
-                    "hb_inspect_model_ex", "hb_selftest_pos_attention"]
+                    "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch"]
+HB_FWD_DEVICE_PTRS = 1
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
@@ -220,6 +222,7 @@ class Context:
         if rc != 0:
             raise HerroError(rc, self._L.hb_last_error(None).decode())
         self.window_size = window_size
+        self.device = device
         self._keep = []
         self.read_len = None
         self.failed = []
@@ -287,6 +290,57 @@ class Context:
 
     def flush(self):
         self._check(self._L.hb_flush(self._h))
+
+    # -- the model call alone -----------------------------------------------------------
+    def forward_batch(self, bases, quals, lens, indices):
+        """The reference's inference() (src/inference.rs:147-175) on one collated batch (hb_forward_batch), with the arguments of
+        oracle/forward_ref.run_batch: bases / quals [B, Lmax, 31] u8 (tokens / raw quality bytes), lens [B], indices: B sequences
+        of rows.  numpy arrays are read from host memory; torch.uint8 CUDA tensors on the context's device are read in place,
+        after the work already queued on torch's current stream.  -> (info logits, bases logits), each a list of B arrays split
+        by lens: numpy float32 arrays, or CUDA tensors for CUDA inputs."""
+        on_device = type(bases).__module__.split(".")[0] == "torch"
+        if on_device:
+            import torch
+            for name, t in (("bases", bases), ("quals", quals)):
+                if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or not t.is_cuda:
+                    raise TypeError(f"{name} must be a torch.uint8 CUDA tensor (or both numpy uint8 arrays)")
+                if t.device.index != self.device:
+                    raise ValueError(f"{name} is on {t.device}, the context on cuda:{self.device}")
+                if not t.is_contiguous():
+                    raise ValueError(f"{name} must be contiguous")
+        else:
+            for name, a in (("bases", bases), ("quals", quals)):
+                if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+                    raise TypeError(f"{name} must be a numpy uint8 array (or both torch.uint8 CUDA tensors)")
+                if not a.flags.c_contiguous:
+                    raise ValueError(f"{name} must be C-contiguous")
+        shape = tuple(bases.shape)
+        if len(shape) != 3 or shape[2] != 31 or tuple(quals.shape) != shape:
+            raise ValueError(f"bases and quals must both be [B, Lmax, 31], got {tuple(bases.shape)} and {tuple(quals.shape)}")
+        B, Lmax = int(shape[0]), int(shape[1])
+        lens = np.ascontiguousarray(np.asarray(lens), dtype=np.int32).reshape(-1)
+        if len(lens) != B or len(indices) != B:
+            raise ValueError(f"lens and indices must have B = {B} entries, got {len(lens)} and {len(indices)}")
+        idx = [np.asarray(i, dtype=np.int32).reshape(-1) for i in indices]
+        for b, i in enumerate(idx):
+            if len(i) != lens[b]:
+                raise ValueError(f"window {b}: lens says {int(lens[b])} positions, indices has {len(i)}")
+        flat = np.ascontiguousarray(np.concatenate(idx) if idx else np.zeros(0, np.int32), dtype=np.int32)
+        n = len(flat)
+        sizes = [int(x) for x in lens]
+        if on_device:
+            info = torch.empty(max(n, 1), dtype=torch.float32, device=bases.device)
+            bl = torch.empty((max(n, 1), 5), dtype=torch.float32, device=bases.device)
+            stream = torch.cuda.current_stream(bases.device).cuda_stream
+            self._check(self._L.hb_forward_batch(self._h, B, Lmax, bases.data_ptr(), quals.data_ptr(), lens.ctypes.data, flat.ctypes.data,
+                                                 info.data_ptr(), bl.data_ptr(), HB_FWD_DEVICE_PTRS, stream))
+            return list(torch.split(info[:n], sizes)), list(torch.split(bl[:n], sizes))
+        info = np.zeros(max(n, 1), np.float32)
+        bl = np.zeros((max(n, 1), 5), np.float32)
+        self._check(self._L.hb_forward_batch(self._h, B, Lmax, bases.ctypes.data, quals.ctypes.data, lens.ctypes.data, flat.ctypes.data,
+                                             info.ctypes.data, bl.ctypes.data, 0, None))
+        cut = np.cumsum(sizes)[:-1]
+        return np.split(info[:n], cut), np.split(bl[:n], cut)
 
     def set_launch_targets(self, n: int):
         self._check(self._L.hb_set_launch_targets(self._h, n))

@@ -3,6 +3,7 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
 
     python -m herro_b200.cli inference --read-alns <dir> -t 4 -d 0 -m model.hbw -b 64 reads.fastq out.fasta
     python -m herro_b200.cli features  --read-alns <dir> -m model.hbw reads.fastq out_dir
+    python -m herro_b200.cli predict   -m model.hbw -b 64 [-d 0] features_dir out_dir   (the model alone, on `features` output)
 
 Nothing is computed here: FASTQ parsing / 2-bit packing, `*.oec.zst` decoding and PAF parsing, the feature / consumer threads
 and the FASTA writer are C++ threads (hbh_inference); `features` drives hb_dump_features launch by launch.  In deployment this
@@ -13,6 +14,7 @@ are not loaded (src/haec_io.rs:48), unknown names / self overlaps / repeated (qu
 from __future__ import annotations
 
 import argparse
+import os
 import sys
 
 from . import api, hostio
@@ -66,6 +68,27 @@ def features(args):
     print(f"Wrote the feature files of {n} reads under {args.output}.", file=sys.stderr)
 
 
+def predict(args):
+    """The model alone on `herro features` output: every read's reference batches (hostio.read_feature_batches) through
+    hb_forward_batch; per window with supported positions, <out>/<read>/<wid>.info_logits.npy (f32 [n]) and
+    <wid>.bases_logits.npy (f32 [n, 5])."""
+    import numpy as np
+    ctx = api.Context(args.model, args.device, batch_size=args.batch_size)
+    n_win = n_pos = 0
+    for read_dir in hostio.feature_reads(args.features):
+        for fb in hostio.read_feature_batches(read_dir, args.batch_size):
+            info, bl = ctx.forward_batch(fb.bases, fb.quals, fb.lens, fb.indices)
+            out = os.path.join(args.output, fb.read)
+            os.makedirs(out, exist_ok=True)
+            for wid, i, b in zip(fb.wids, info, bl):
+                np.save(os.path.join(out, f"{wid}.info_logits.npy"), i)
+                np.save(os.path.join(out, f"{wid}.bases_logits.npy"), b)
+                n_win += 1
+                n_pos += len(i)
+    ctx.close()
+    print(f"Wrote the logits of {n_pos} supported positions in {n_win} windows under {args.output}.", file=sys.stderr)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="herro_b200")
     sub = ap.add_subparsers(dest="cmd", required=True)
@@ -86,9 +109,17 @@ def main(argv=None):
     ft.add_argument("--targets-per-launch", type=int, default=256)
     ft.add_argument("reads")
     ft.add_argument("output")
+    pr = sub.add_parser("predict", help="the model alone on a `features` output directory")
+    pr.add_argument("-m", dest="model", required=True)
+    pr.add_argument("-b", dest="batch_size", type=int, required=True, help="windows per model batch, as `-b` of the features run")
+    pr.add_argument("-d", dest="device", type=int, default=0)
+    pr.add_argument("features")
+    pr.add_argument("output")
     args = ap.parse_args(argv)
     if args.cmd == "inference":
         return inference(args)
+    if args.cmd == "predict":
+        return predict(args)
     return features(args)
 
 

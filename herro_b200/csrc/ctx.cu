@@ -249,6 +249,23 @@ struct hb_ctx {
     uint32_t min_launch = 256;  // smallest per-thread hand-over unless launch_targets itself is smaller (HERRO_B200_MIN_LAUNCH: experiments)
     int last_lane = -1;  // lane of the most recently finished launch (debug taps / replay)
     uint32_t chunk_pos = 65536;  // supported positions per forward pass (HERRO_B200_CHUNK_POS): one pass per launch unless huge
+    // hb_forward_batch's lane: its own stream, events, timer and grow-only scratch, which the launch lanes never touch.  Calls
+    // serialise on its mutex.
+    struct FwdLane {
+        std::mutex mu;
+        cudaStream_t stream = nullptr;
+        cudaEvent_t ev[3]{};  // the caller's stream, forward start, forward end
+        KTimer kt;
+        PinBuf pin_in, pin_out;     // input region (carve_fwd_in) + the work list; the host outputs
+        DevBuf d_in, d_mat, d_fwd;  // input region; the [rows][32] matrices; the forward region (carve_fwd)
+        void release() {
+            d_in.release(); d_mat.release(); d_fwd.release();
+            pin_in.release(); pin_out.release();
+            for (auto& e : ev) if (e) cudaEventDestroy(e);
+            kt.destroy();
+            if (stream) cudaStreamDestroy(stream);
+        }
+    } fwd;
 
     std::deque<Result> results;
     hb_stats stats{};
@@ -699,20 +716,41 @@ int zero_scratch(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b) {
     return HB_OK;
 }
 
-// The forward + consensus part once the supported positions of every window (nsup[nw]) are known.  A forward pass takes
-// as many whole windows as fit in chunk_pos positions; a window larger than that is a pass of its own.
-int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, const uint32_t* nsup, size_t nw, uint64_t* launches) {
-    *launches += launch_features_c2(b, L->stream, L->kt);
-    uint64_t n0 = 0;
+// The forward over the work list of windows [0, nw) (nsup[nw] positions each, back to back).  A forward pass takes as many whole
+// windows as fit in chunk_pos positions; a window larger than that is a pass of its own.  Returns the kernel launches.
+uint64_t launch_forward_passes(const hb_ctx* ctx, const BatchView& b, const FwdBufs& f, const uint32_t* nsup, size_t nw, cudaStream_t st,
+                               KTimer& kt) {
+    uint64_t n0 = 0, launches = 0;
     for (size_t w0 = 0; w0 < nw;) {
         uint64_t np = nsup[w0];
         size_t w1 = w0 + 1;
         while (w1 < nw && np + nsup[w1] <= ctx->chunk_pos) np += nsup[w1++];
-        if (np) *launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, (uint32_t)np, (uint32_t)w0, (uint32_t)(w1 - w0), f.ws, f.logits,
-                                                  f.info, L->stream, L->kt);
+        if (np) launches += launch_forward_chunk(b, ctx->wt, (uint32_t)n0, (uint32_t)np, (uint32_t)w0, (uint32_t)(w1 - w0), f.ws, f.logits,
+                                                 f.info, st, kt);
         n0 += np;
         w0 = w1;
     }
+    return launches;
+}
+
+// Algorithmic FLOPs of the forward at n_sup positions in windows of nsup[nw] positions
+void add_forward_flops(const hb_ctx* ctx, hb_stats& S, uint64_t n_sup, const uint32_t* nsup, size_t nw) {
+    uint64_t gf = 0;
+    const uint64_t ff = forward_flops_per_pos(ctx->wt, &gf);
+    S.forward_flops += ff * n_sup;
+    S.gemm_flops += gf * n_sup;
+    uint64_t cf[16];
+    forward_class_flops_per_pos(ctx->wt, cf);
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) S.class_flops[i] += cf[i] * n_sup;
+    const uint64_t pa = pos_attn_flops(ctx->wt, nsup, nw);
+    S.class_flops[K_POS_ATTN] += pa;
+    S.forward_flops += pa;
+}
+
+// The forward + consensus part once the supported positions of every window (nsup[nw]) are known.
+int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, const uint32_t* nsup, size_t nw, uint64_t* launches) {
+    *launches += launch_features_c2(b, L->stream, L->kt);
+    *launches += launch_forward_passes(ctx, b, f, nsup, nw, L->stream, L->kt);
     CK(cudaEventRecord(L->ev[4], L->stream));
     *launches += launch_consensus(b, L->stream, L->kt);
     CK(cudaEventRecord(L->ev[5], L->stream));
@@ -814,18 +852,7 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     cudaEventElapsedTime(&ms, L->ev[4], L->ev[5]); S.ms_consensus += ms;
     L->kt.collect(S.ms_kernel, S.n_kernel);
     L->kt.on = false;
-    {
-        uint64_t gf = 0;
-        const uint64_t ff = forward_flops_per_pos(ctx->wt, &gf);
-        S.forward_flops += ff * n_sup;
-        S.gemm_flops += gf * n_sup;
-        uint64_t cf[16];
-        forward_class_flops_per_pos(ctx->wt, cf);
-        for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) S.class_flops[i] += cf[i] * n_sup;
-        const uint64_t pa = pos_attn_flops(ctx->wt, h.nsup, nw);
-        S.class_flops[K_POS_ATTN] += pa;
-        S.forward_flops += pa;
-    }
+    add_forward_flops(ctx, S, n_sup, h.nsup, nw);
 
     // ---- per-read reassembly (src/consensus.rs:90-111,222-226)
     const uint8_t* outb = L->pin_out.as<uint8_t>();
@@ -1257,6 +1284,176 @@ int stage_target(hb_ctx* ctx, const PreparedTarget& P, const hb_overlap* ovl, ui
     return HB_OK;
 }
 
+// ---------------------------------------------------------------------------------- hb_forward_batch
+// Its input region: the caller's tokens and qualities (host path only: in_bytes is 0 otherwise), the per-window arrays of the
+// view and the error word.  Carved alike in pinned and in device memory, so one copy moves all of it.
+struct FwdIn {
+    uint8_t *tok, *qual;
+    uint32_t *L, *nsup, *nsel;
+    uint64_t *rowbase, *supbase;
+    unsigned long long* bad;
+};
+size_t carve_fwd_in(FwdIn& a, size_t in_bytes, size_t nb, uint8_t* base) {
+    Carve c{base};
+    c(a.tok, in_bytes);
+    c(a.qual, in_bytes);
+    c(a.L, nb);
+    c(a.nsup, nb);
+    c(a.nsel, nb);
+    c(a.rowbase, nb);
+    c(a.supbase, nb);
+    c(a.bad, 1);
+    return c.bytes;
+}
+
+// Where a caller's pointer lives: 1 device memory of `device` (or managed), -1 another device's memory, 0 host memory
+int pointer_kind(const void* p, int device) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (at.type == cudaMemoryTypeManaged) return 1;
+    if (at.type != cudaMemoryTypeDevice) return 0;
+    return at.device == device ? 1 : -1;
+}
+
+// The work of hb_forward_batch, with the lane's lock held and the context's device current
+int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
+                  const int32_t* indices, float* info_out, float* logits_out, uint32_t flags, void* stream) {
+    hb_ctx::FwdLane& F = ctx->fwd;
+    if (!bases || !quals || !lens || !indices || !info_out || !logits_out) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (B == 0 || Lmax == 0) return fail(ctx, HB_ERR_ARG, "B and Lmax must be positive");
+    if (flags & ~HB_FWD_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
+    const bool dev = (flags & HB_FWD_DEVICE_PTRS) != 0;
+    {
+        const void* p[6] = {bases, quals, info_out, logits_out, lens, indices};
+        static const char* name[6] = {"bases", "quals", "info_logits", "bases_logits", "lens", "indices"};
+        for (int i = 0; i < 6; i++) {
+            const int k = pointer_kind(p[i], ctx->device);
+            if (dev && i < 4 && k != 1)
+                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is not memory of device " + std::to_string(ctx->device) +
+                                                 " (HB_FWD_DEVICE_PTRS is set)");
+            if ((!dev || i >= 4) && k != 0)
+                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is device memory" + (i < 4 ? " (HB_FWD_DEVICE_PTRS is not set)" : ""));
+        }
+    }
+    uint64_t n = 0;
+    uint32_t max_len = 0;
+    for (uint32_t b = 0; b < B; b++) {
+        if (lens[b] < 0) return fail(ctx, HB_ERR_ARG, "lens[" + std::to_string(b) + "] is negative");
+        n += (uint64_t)lens[b];
+        max_len = std::max(max_len, (uint32_t)lens[b]);
+    }
+    if (n == 0) return HB_OK;
+    const uint64_t rows = (uint64_t)B * Lmax;
+    if (n >= (1ull << 31) || rows >= (1ull << 36)) return fail(ctx, HB_ERR_CAPACITY, "batch too large");
+    // ---- scratch (grow-only) and the view
+    const size_t in_bytes = dev ? 0 : (size_t)rows * R_COLS;
+    FwdIn hp, dp;
+    const size_t in_sz = carve_fwd_in(hp, in_bytes, B, nullptr);
+    CK(F.pin_in.grow(in_sz + 2 * al256(n * 4)));
+    carve_fwd_in(hp, in_bytes, B, F.pin_in.as<uint8_t>());
+    uint32_t* h_win = (uint32_t*)(F.pin_in.as<uint8_t>() + in_sz);
+    uint32_t* h_row = (uint32_t*)((uint8_t*)h_win + al256(n * 4));
+    CK(F.d_in.grow(in_sz));
+    carve_fwd_in(dp, in_bytes, B, F.d_in.as<uint8_t>());
+    BatchView b{};
+    b.n_win = B;
+    b.w_L = b.w_reflmax = dp.L;  // every window is Lmax rows long, and so is its batch
+    b.w_nsup = dp.nsup;
+    b.w_nsel = dp.nsel;          // 0: k_heads writes no consensus byte
+    b.w_rowbase = dp.rowbase;
+    b.w_supbase = dp.supbase;
+    CK(F.d_mat.grow(2 * al256(rows * ROW_BYTES)));
+    b.mat_bases = F.d_mat.as<uint8_t>();
+    b.mat_quals = b.mat_bases + al256(rows * ROW_BYTES);
+    FwdBufs f;
+    CK(F.d_fwd.grow(carve_fwd(ctx, b, f, n, max_len, nullptr)));
+    carve_fwd(ctx, b, f, n, max_len, F.d_fwd.as<uint8_t>());
+    float *h_info = nullptr, *h_logits = nullptr;
+    if (!dev) {
+        CK(F.pin_out.grow(al256(n * 4) + n * 20));
+        h_info = F.pin_out.as<float>();
+        h_logits = (float*)(F.pin_out.as<uint8_t>() + al256(n * 4));
+    }
+    // ---- the per-window arrays and the work list, checking every index
+    uint64_t sb = 0;
+    for (uint32_t w = 0; w < B; w++) {
+        hp.L[w] = Lmax;
+        hp.nsup[w] = (uint32_t)lens[w];
+        hp.nsel[w] = 0;
+        hp.rowbase[w] = (uint64_t)w * Lmax;
+        hp.supbase[w] = sb;
+        for (uint32_t k = 0; k < (uint32_t)lens[w]; k++) {
+            const int32_t r = indices[sb + k];
+            if (r < 0 || (uint32_t)r >= Lmax)
+                return fail(ctx, HB_ERR_ARG, "indices[" + std::to_string(sb + k) + "] = " + std::to_string(r) + " (window " + std::to_string(w) +
+                                                 ") is outside [0, Lmax = " + std::to_string(Lmax) + ")");
+            h_win[sb + k] = w;
+            h_row[sb + k] = (uint32_t)r;
+        }
+        sb += (uint32_t)lens[w];
+    }
+    *hp.bad = ~0ull;
+    if (!dev) {
+        memcpy(hp.tok, bases, in_bytes);
+        memcpy(hp.qual, quals, in_bytes);
+    }
+    // ---- device work
+    KTimer& kt = F.kt;
+    kt.discard();
+    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
+    kt.st = F.stream;
+    if (dev) {
+        CK(cudaEventRecord(F.ev[0], (cudaStream_t)stream));
+        CK(cudaStreamWaitEvent(F.stream, F.ev[0], 0));
+    }
+    CK(cudaMemcpyAsync(F.d_in.p, F.pin_in.p, in_sz, cudaMemcpyHostToDevice, F.stream));
+    CK(cudaMemcpyAsync(b.fwd_win, h_win, n * 4, cudaMemcpyHostToDevice, F.stream));
+    CK(cudaMemcpyAsync(b.fwd_row, h_row, n * 4, cudaMemcpyHostToDevice, F.stream));
+    CK(cudaEventRecord(F.ev[1], F.stream));
+    kt.begin(K_LISTS);
+    launch_batch_in(dev ? bases : dp.tok, dev ? quals : dp.qual, rows, b.mat_bases, b.mat_quals, dp.bad, F.stream);
+    kt.end();
+    const uint64_t launches = 1 + launch_forward_passes(ctx, b, f, hp.nsup, B, F.stream, kt);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(F.ev[2], F.stream));
+    CK(cudaMemcpyAsync(hp.bad, dp.bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, F.stream));
+    if (!dev) {
+        CK(cudaMemcpyAsync(h_info, f.info, n * 4, cudaMemcpyDeviceToHost, F.stream));
+        CK(cudaMemcpyAsync(h_logits, f.logits, n * 20, cudaMemcpyDeviceToHost, F.stream));
+    }
+    CK(cudaStreamSynchronize(F.stream));
+    if (*hp.bad != ~0ull) {
+        kt.discard();
+        const uint64_t e = *hp.bad, per = (uint64_t)Lmax * R_COLS;
+        return fail(ctx, HB_ERR_INPUT, "token above 11 at (b, row, col) = (" + std::to_string(e / per) + ", " + std::to_string(e % per / R_COLS) +
+                                            ", " + std::to_string(e % R_COLS) + "): the model's embedding has 12 entries");
+    }
+    if (dev) {
+        CK(cudaMemcpyAsync(info_out, f.info, n * 4, cudaMemcpyDeviceToDevice, F.stream));
+        CK(cudaMemcpyAsync(logits_out, f.logits, n * 20, cudaMemcpyDeviceToDevice, F.stream));
+        CK(cudaStreamSynchronize(F.stream));
+    } else {
+        memcpy(info_out, h_info, n * 4);
+        memcpy(logits_out, h_logits, n * 20);
+    }
+    // ---- counters
+    hb_stats S{};
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, F.ev[1], F.ev[2]));
+    kt.collect(S.ms_kernel, S.n_kernel);
+    kt.on = false;
+    add_forward_flops(ctx, S, n, hp.nsup, B);
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    hb_stats& T = ctx->stats;
+    T.ms_forward += ms;
+    T.supported += n;
+    T.kernel_launches += launches;
+    T.gemm_flops += S.gemm_flops;
+    T.forward_flops += S.forward_flops;
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; T.class_flops[i] += S.class_flops[i]; }
+    return HB_OK;
+}
+
 }  // namespace
 
 // ========================================================================================
@@ -1340,6 +1537,13 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
             if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
         L.d_batch.st = L.d_rows.st = L.d_fwd.st = L.stream;
     }
+    {
+        auto& F = ctx->fwd;
+        if (cudaStreamCreateWithFlags(&F.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
+        for (auto& e : F.ev)
+            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
+        F.d_in.st = F.d_mat.st = F.d_fwd.st = F.stream;
+    }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
         cudaMemPool_t pool;
         uint64_t keep = UINT64_MAX;
@@ -1365,10 +1569,12 @@ void hb_destroy(hb_ctx* ctx) {
     for (auto& L : ctx->lanes) if (L.worker.joinable()) L.worker.join();
     cudaSetDevice(ctx->device);
     for (auto& L : ctx->lanes) if (L.stream) cudaStreamSynchronize(L.stream);
+    if (ctx->fwd.stream) cudaStreamSynchronize(ctx->fwd.stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
     DevBuf* bufs[] = {&ctx->d_words, &ctx->d_word_off, &ctx->d_len, &ctx->d_qual, &ctx->d_qual_off, &ctx->d_ln};
     for (DevBuf* b : bufs) b->release();
     for (auto& L : ctx->lanes) L.release();
+    ctx->fwd.release();
     ctx->pin_in.release();
     ctx->slots.clear();
     ctx->queue.clear();
@@ -1951,6 +2157,25 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
     L->kt.discard();
     ctx->stats.kernel_launches += launches;
     return HB_OK;
+}
+
+int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
+                     const int32_t* indices, float* info_logits, float* bases_logits, uint32_t flags, void* stream) {
+    if (!ctx) return HB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->fwd.mu);
+    int prev = -1;
+    cudaGetDevice(&prev);
+    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
+    t_err_sink = &err;
+    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
+    if (rc == HB_OK) rc = forward_batch(ctx, B, Lmax, bases, quals, lens, indices, info_logits, bases_logits, flags, stream);
+    t_err_sink = nullptr;
+    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
+    if (rc != HB_OK) {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        ctx->err = err;
+    }
+    return rc;
 }
 
 }  // extern "C"

@@ -172,6 +172,11 @@ uint64_t pos_attn_flops(const FwdWeights& wt, const uint32_t* nsup, size_t nwin)
 // algorithmic FLOPs per supported position attributed to the kernel class that executes them on the active code path
 void forward_class_flops_per_pos(const FwdWeights& wt, uint64_t (&out)[16]);
 
+// batch_in.cu: a caller's [rows][31] tokens and quality bytes (any alignment) -> the [rows][32] matrices, column 31 = token 10 /
+// quality 33; a token above 11 is written as 0xff (contributes nothing) and the smallest linear index of one is atomicMin'ed into *bad
+void launch_batch_in(const uint8_t* tok, const uint8_t* qual, uint64_t rows, uint8_t* mat_b, uint8_t* mat_q, unsigned long long* bad,
+                     cudaStream_t st);
+
 // features.cu
 cudaError_t features_configure(uint32_t W);
 int launch_features_a(const BatchView& b, cudaStream_t st, KTimer& kt);

@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from dataclasses import dataclass
 
 import numpy as np
 
@@ -172,6 +173,68 @@ class FastaWriter:
             self._H.hbh_fasta_close(self._h, C.byref(rec), C.byref(bases))
             self._h = C.c_void_p()
         return rec.value, bases.value
+
+
+# ------------------------------------------------------------------------------------------
+# `herro features` directories (src/features.rs:724-764) -> the reference's model batches (src/inference.rs:73-140,222-268)
+# ------------------------------------------------------------------------------------------
+BASES_MAP = np.full(256, 255, dtype=np.uint8)  # src/inference.rs:23-31: ASCII -> token, 255 elsewhere
+for _tok, _ch in enumerate(b"ACGT*acgt#."):
+    BASES_MAP[_ch] = _tok
+TOK_GAP = 4          # BASES_MAP['*']: a row whose target column holds it is an insertion row
+BASE_PADDING, QUAL_PADDING = 11, 126  # src/inference.rs:15-17
+
+
+@dataclass
+class FeatureBatch:
+    """One collated reference batch of a read: the arguments of inference() (src/inference.rs:147-175)."""
+    read: str
+    wids: list           # [B] window ids, the batch's window order
+    bases: np.ndarray    # [B, Lmax, 31] u8 tokens, padded with 11
+    quals: np.ndarray    # [B, Lmax, 31] u8 quality bytes, padded with 126
+    lens: np.ndarray     # [B] i32 supported positions per window
+    indices: list        # B arrays of i32 rows: target_rows[pos] + ins
+
+
+def read_feature_window(read_dir: str, wid: int):
+    """-> (tokens [L, 31] u8, quals [L, 31] u8, indices [n] i32) of one window of a `herro features` read directory."""
+    feats = np.load(os.path.join(read_dir, f"{wid}.features.npy"))
+    sup = np.load(os.path.join(read_dir, f"{wid}.supported.npy"))
+    if feats.ndim != 3 or feats.shape[0] != 2 or feats.shape[2] != 31:
+        raise ValueError(f"{read_dir}/{wid}.features.npy: expected [2, L, 31], got {feats.shape}")
+    tok = BASES_MAP[feats[0]]
+    target_rows = np.flatnonzero(tok[:, 0] != TOK_GAP)                   # get_target_indices (:255-268)
+    idx = target_rows[sup["pos"].astype(np.int64)] + sup["ins"].astype(np.int64)  # (:136-140)
+    return tok, np.ascontiguousarray(feats[1]), idx.astype(np.int32)
+
+
+def read_feature_batches(read_dir: str, batch_size: int):
+    """The model batches of one read directory, in the order the reference runs them: the windows in wid order are taken `batch_size`
+    at a time, as FeaturesOutput::update hands them over (src/features.rs:884-893); the windows of such a group with at least one
+    supported position form one batch (prepare_examples, src/inference.rs:241-250), padded to its longest window (collate, :73-97)."""
+    wids = sorted(int(f[:-len(".features.npy")]) for f in os.listdir(read_dir) if f.endswith(".features.npy"))
+    read = os.path.basename(os.path.normpath(read_dir))
+    out = []
+    for g0 in range(0, len(wids), batch_size):
+        wins = [(w,) + read_feature_window(read_dir, w) for w in wids[g0:g0 + batch_size]]
+        wins = [w for w in wins if len(w[3]) > 0]
+        if not wins:
+            continue
+        lmax = max(w[1].shape[0] for w in wins)
+        bases = np.full((len(wins), lmax, 31), BASE_PADDING, dtype=np.uint8)
+        quals = np.full((len(wins), lmax, 31), QUAL_PADDING, dtype=np.uint8)
+        for b, (_, tok, q, _) in enumerate(wins):
+            bases[b, :tok.shape[0]] = tok
+            quals[b, :q.shape[0]] = q
+        out.append(FeatureBatch(read, [w[0] for w in wins], bases, quals, np.array([len(w[3]) for w in wins], dtype=np.int32),
+                                [w[3] for w in wins]))
+    return out
+
+
+def feature_reads(features_dir: str):
+    """The read directories of a `herro features` output directory (those holding window files), sorted by name."""
+    return [os.path.join(features_dir, d) for d in sorted(os.listdir(features_dir))
+            if os.path.isdir(os.path.join(features_dir, d)) and any(f.endswith(".features.npy") for f in os.listdir(os.path.join(features_dir, d)))]
 
 
 def inference(reads_path: str, alns_dir: str, model: str, output: str, window: int = 4096, batch: int = 64, threads: int = 1,

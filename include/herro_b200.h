@@ -121,6 +121,45 @@ int hb_submit_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_ove
  * (inverted ranges, windows past the end of the target) still fail here. */
 int hb_submit_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_t n_ovl);
 
+/* ---- the model call alone ---------------------------------------------------------------- */
+#define HB_FWD_DEVICE_PTRS 1u  /* bases, quals and both outputs are device pointers on the context's device */
+/* The replacement of inference() (src/inference.rs:147-175) on one collated batch, for a host that keeps its own features stage,
+ * batching and consensus.
+ *
+ *   bases, quals   [B][Lmax][31] u8, C order: BASES_MAP tokens (src/inference.rs:23-31) / raw quality bytes
+ *   lens           [B] i32, host memory: supported positions of each window
+ *   indices        [sum lens] i32, host memory: the rows of window b's positions, window after window
+ *   info_logits    [sum lens] f32, bases_logits [sum lens][5] f32: in `indices` order
+ *   stream         with HB_FWD_DEVICE_PTRS: the cudaStream_t whose pending work produces the inputs (NULL: the legacy default stream)
+ *
+ * What it computes: the model's graph over the whole tensor, as collate + forward_is do.  Rows [0, Lmax) are taken as given,
+ * wherever token 11 (the batch padding) appears; rows outside [0, Lmax) contribute nothing (the conv's zero padding).  The
+ * qualities are normalised on the device as inference() does, fl(fl(q * fl(2/93)) - fl(66/93 + 1)), for any byte 0-255.  A model
+ * with the encoder stage across positions attends within each of the B windows.  Nothing of consensus runs.
+ *
+ * Synchronous: returns when the outputs are written.  With HB_FWD_DEVICE_PTRS the library's stream first waits, through an event,
+ * for the work already enqueued on `stream`; host inputs and outputs go through pinned staging that only grows, so repeated
+ * calls of the same or smaller shape allocate nothing.
+ *
+ * Errors (the context stays usable for the pipeline and the next call; nothing is written to the outputs):
+ *   HB_ERR_ARG       a NULL pointer, B == 0 or Lmax == 0, a negative length, an index outside [0, Lmax), or a pointer that does
+ *                    not match the flag (with it: host memory or another device's memory; without it: device memory)
+ *   HB_ERR_INPUT     a token above 11 (the reference's Embedding would raise); the message names the first offending (b, row, col)
+ *                    in row-major order
+ *   HB_ERR_CAPACITY  scratch could not grow
+ *   HB_ERR_CUDA      a CUDA failure
+ * sum lens == 0 is HB_OK and writes nothing.  Duplicated and unsorted indices are fine.
+ *
+ * Threading: may be called from any thread, concurrently with hb_submit_*, hb_flush and hb_poll_corrected on the same context;
+ * calls of hb_forward_batch on one context serialise among themselves.  It needs no hb_upload_reads, and never touches the
+ * pipeline's scratch, the debug taps or the launch hb_replay_last_launch re-runs.
+ *
+ * Counters: adds to kernel_launches, n_kernel / ms_kernel (the input kernel under HB_K_LISTS), ms_forward, supported, the FLOP
+ * counters (per position, as the pipeline counts them) and host_allocs when scratch grows; targets, windows, rows and
+ * corrected_bases are untouched. */
+int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
+                     const int32_t* indices, float* info_logits, float* bases_logits, uint32_t flags, void* stream);
+
 /* Host-only utility: the windows [*first_window, *end_window) one alignment contributes OverlapWindows to — the
  * coordinate-only part of extract_windows (src/windowing.rs:53-125,260-272).  HB_ERR_INPUT where the reference panics. */
 int hb_window_range(const hb_overlap* ovl, uint32_t window_size, uint32_t n_windows, uint32_t* first_window, uint32_t* end_window);
