@@ -104,6 +104,7 @@ def load_library():
     L.hb_selftest_gemm.argtypes = [C.c_int, u32, u32, u32, C.c_int, C.c_int, u32, fp, fp, fp, fp]
     L.hb_selftest_pos_attention.argtypes = [C.c_int, u32p, u32, u32, u32, fp, fp, fp]
     L.hb_forward_batch.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp, vp, u32, vp]
+    L.hb_consensus_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u32, vp]
     _lib = L
     return L
 
@@ -111,8 +112,9 @@ def load_library():
 EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "hb_bind_calling_thread", "hb_set_launch_targets", "hb_set_kernel_timing", "hb_extract_windows", "hb_create", "hb_destroy", "hb_upload_reads", "hb_submit_target", "hb_submit_alignments", "hb_flush",
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
-                    "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch"]
+                    "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch"]
 HB_FWD_DEVICE_PTRS = 1
+HB_CONS_DEVICE_PTRS = 1
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
@@ -341,6 +343,82 @@ class Context:
                                              info.ctypes.data, bl.ctypes.data, 0, None))
         cut = np.cumsum(sizes)[:-1]
         return np.split(info[:n], cut), np.split(bl[:n], cut)
+
+    # -- consensus alone ----------------------------------------------------------------
+    def consensus_batch(self, n_windows, rows, n_alns, bases, supported, bases_logits):
+        """The reference's consensus() (src/consensus.rs:86-227) on the windows of several reads (hb_consensus_batch).
+        n_windows: windows per read (all of a read's windows, in wid order); rows, n_alns: per window; bases [sum rows, 31] u8
+        tokens, window after window; supported: per window a [n, 2] array of (pos, ins); bases_logits [sum n, 5] f32, one row per
+        supported entry in the same order.  bases and bases_logits are both numpy arrays, or both CUDA tensors on the context's
+        device (read after the work already queued on torch's current stream).  -> per read, a list of bytes segments (empty: the
+        read gets no record)."""
+        on_device = type(bases).__module__.split(".")[0] == "torch"
+        if on_device:
+            import torch
+            for name, t, dt in (("bases", bases, torch.uint8), ("bases_logits", bases_logits, torch.float32)):
+                if not isinstance(t, torch.Tensor) or t.dtype != dt or not t.is_cuda:
+                    raise TypeError(f"{name} must be a {dt} CUDA tensor (or both numpy arrays)")
+                if t.device.index != self.device:
+                    raise ValueError(f"{name} is on {t.device}, the context on cuda:{self.device}")
+                if not t.is_contiguous():
+                    raise ValueError(f"{name} must be contiguous")
+        else:
+            for name, a, dt in (("bases", bases, np.uint8), ("bases_logits", bases_logits, np.float32)):
+                if not isinstance(a, np.ndarray) or a.dtype != dt:
+                    raise TypeError(f"{name} must be a numpy {np.dtype(dt).name} array (or both CUDA tensors)")
+                if not a.flags.c_contiguous:
+                    raise ValueError(f"{name} must be C-contiguous")
+
+        def counts(name, x, hi):
+            a = np.asarray(x).reshape(-1)
+            if a.size and (a.dtype.kind not in "iu" or int(a.min()) < 0 or int(a.max()) > hi):
+                raise ValueError(f"{name} must hold integers in [0, {hi}]")
+            return np.ascontiguousarray(a, dtype=np.uint8 if hi == 255 else np.uint32)
+
+        nwin = counts("n_windows", n_windows, 0xffffffff)
+        W = int(nwin.sum())
+        rows_a, nal = counts("rows", rows, 0xffffffff), counts("n_alns", n_alns, 255)
+        if len(rows_a) != W or len(nal) != W or len(supported) != W:
+            raise ValueError(f"rows, n_alns and supported must have one entry per window ({W}), got {len(rows_a)}, {len(nal)} and {len(supported)}")
+        sup = [counts("supported", s, 0xffffffff).reshape(-1, 2) if np.asarray(s).size else np.zeros((0, 2), np.uint32) for s in supported]
+        for w, s in enumerate(supported):
+            if np.asarray(s).size and np.asarray(s).shape[-1] != 2:
+                raise ValueError(f"supported[{w}] must be [n, 2] (pos, ins), got {np.asarray(s).shape}")
+        nsup = np.array([len(s) for s in sup], dtype=np.uint32)
+        N, S = int(rows_a.astype(np.uint64).sum()), int(nsup.sum())
+        if tuple(bases.shape) != (N, 31):
+            raise ValueError(f"bases must be [sum rows = {N}, 31], got {tuple(bases.shape)}")
+        if tuple(bases_logits.shape) != (S, 5):
+            raise ValueError(f"bases_logits must be [sum supported = {S}, 5], got {tuple(bases_logits.shape)}")
+        flat = np.ascontiguousarray(np.concatenate(sup) if sup else np.zeros((0, 2), np.uint32), dtype=np.uint32)
+        n_reads = len(nwin)
+        seqs = np.zeros(max(N, 1), np.uint8)
+        seg_len = np.zeros(max(W, 1), np.uint32)
+        n_segs = np.zeros(max(n_reads, 1), np.uint32)
+        keep = [nwin, rows_a, nal, nsup, flat]
+        ptrs = [a.ctypes.data if a.size else np.zeros(1, np.uint32).ctypes.data for a in keep]
+        keep.append(ptrs)
+        if on_device:  # an empty tensor may have no storage: the library wants a pointer of the device all the same
+            b = bases if N else torch.zeros((1, 31), dtype=torch.uint8, device=bases.device)
+            bl = bases_logits if S else torch.zeros((1, 5), dtype=torch.float32, device=bases.device)
+            stream = torch.cuda.current_stream(bases.device).cuda_stream
+            self._check(self._L.hb_consensus_batch(self._h, n_reads, ptrs[0], ptrs[1], ptrs[2], b.data_ptr(), ptrs[3], ptrs[4],
+                                                   bl.data_ptr(), seqs.ctypes.data, seg_len.ctypes.data, n_segs.ctypes.data,
+                                                   HB_CONS_DEVICE_PTRS, stream))
+        else:
+            b = bases if N else np.zeros((1, 31), np.uint8)
+            bl = bases_logits if S else np.zeros((1, 5), np.float32)
+            self._check(self._L.hb_consensus_batch(self._h, n_reads, ptrs[0], ptrs[1], ptrs[2], b.ctypes.data, ptrs[3], ptrs[4],
+                                                   bl.ctypes.data, seqs.ctypes.data, seg_len.ctypes.data, n_segs.ctypes.data, 0, None))
+        out, s, o = [], 0, 0
+        for i in range(n_reads):
+            segs = []
+            for _ in range(int(n_segs[i])):
+                segs.append(seqs[o:o + int(seg_len[s])].tobytes())
+                o += int(seg_len[s])
+                s += 1
+            out.append(segs)
+        return out
 
     def set_launch_targets(self, n: int):
         self._check(self._L.hb_set_launch_targets(self._h, n))

@@ -4,6 +4,8 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
     python -m herro_b200.cli inference --read-alns <dir> -t 4 -d 0 -m model.hbw -b 64 reads.fastq out.fasta
     python -m herro_b200.cli features  --read-alns <dir> -m model.hbw reads.fastq out_dir
     python -m herro_b200.cli predict   -m model.hbw -b 64 [-d 0] features_dir out_dir   (the model alone, on `features` output)
+    python -m herro_b200.cli consensus -m model.hbw [-d 0] features_dir logits_dir reads.fastq out.fasta
+                                       (consensus alone, on `features` and `predict` output)
 
 Nothing is computed here: FASTQ parsing / 2-bit packing, `*.oec.zst` decoding and PAF parsing, the feature / consumer threads
 and the FASTA writer are C++ threads (hbh_inference); `features` drives hb_dump_features launch by launch.  In deployment this
@@ -89,6 +91,40 @@ def predict(args):
     print(f"Wrote the logits of {n_pos} supported positions in {n_win} windows under {args.output}.", file=sys.stderr)
 
 
+def consensus(args):
+    """consensus() alone on `features` and `predict` output: every read's ConsensusWindows (hostio.read_consensus_windows) through
+    hb_consensus_batch, many reads per call, written as correction_writer writes them.  The FASTQ gives only ids and descriptions."""
+    R = hostio.Reads(args.reads, min_len=0)
+    desc = dict(zip(R.ids, R.descriptions))
+    R.close()
+    ctx = api.Context(args.model, args.device)
+    out = hostio.FastaWriter(args.output)
+    pending, rows = [], 0
+
+    def run():
+        names = [n for n, _ in pending]
+        for name, segs in zip(names, ctx.consensus_batch(*hostio.consensus_args([w for _, w in pending]))):
+            if segs:
+                out.write(name, desc.get(name), segs)
+        pending.clear()
+
+    for read_dir in hostio.feature_reads(args.features):
+        name = os.path.basename(read_dir)
+        wins = hostio.read_consensus_windows(read_dir, os.path.join(args.logits, name))
+        if name.encode() not in desc:
+            raise SystemExit(f"read {name} of {args.features} is not in {args.reads}")
+        pending.append((name.encode(), wins))
+        rows += sum(w.bases.shape[0] for w in wins)
+        if rows >= args.rows_per_call:
+            run()
+            rows = 0
+    if pending:
+        run()
+    records, bases = out.close()
+    ctx.close()
+    print(f"Wrote {records} records ({bases} bases) to {args.output}.", file=sys.stderr)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="herro_b200")
     sub = ap.add_subparsers(dest="cmd", required=True)
@@ -115,11 +151,21 @@ def main(argv=None):
     pr.add_argument("-d", dest="device", type=int, default=0)
     pr.add_argument("features")
     pr.add_argument("output")
+    cs = sub.add_parser("consensus", help="consensus alone on `features` and `predict` output directories")
+    cs.add_argument("-m", dest="model", required=True, help="weights (a context needs them; consensus does not use them)")
+    cs.add_argument("-d", dest="device", type=int, default=0)
+    cs.add_argument("--rows-per-call", type=int, default=1 << 22, help="window rows gathered before each library call")
+    cs.add_argument("features")
+    cs.add_argument("logits")
+    cs.add_argument("reads")
+    cs.add_argument("output")
     args = ap.parse_args(argv)
     if args.cmd == "inference":
         return inference(args)
     if args.cmd == "predict":
         return predict(args)
+    if args.cmd == "consensus":
+        return consensus(args)
     return features(args)
 
 

@@ -7,39 +7,14 @@
 // column 31 set to the pad byte k_pileup writes (token 10, quality 33).  HBM-bound: 2·B·Lmax·(31 + 32) bytes per call.
 #include "common.cuh"
 #include "forward.h"
+#include "tile.cuh"
 
 namespace hb {
 
 namespace {
 
-constexpr int BI_ROWS = 256;                         // rows per block, one per thread
-constexpr int BI_WORDS = (BI_ROWS * R_COLS + 3) / 4 + 2;  // a tile's bytes at any misalignment, plus the word a row's last shift reads
-
-// Words [0, nw) of the tile that starts at `lo` (nb bytes, `mis` bytes past an aligned address) into s.  A word that lies wholly
-// inside the tile is loaded as a word; the others are assembled from the tile's bytes, zero outside it.
-__device__ __forceinline__ void stage_tile(uint32_t* s, const uint8_t* __restrict__ lo, uint32_t nb, uint32_t mis) {
-    const uint32_t* wbase = (const uint32_t*)(lo - mis);
-    const uint32_t nw = (mis + nb + 3) / 4 + 1;
-    for (uint32_t i = threadIdx.x; i < nw; i += blockDim.x) {
-        const uint32_t b0 = 4 * i;
-        uint32_t v = 0;
-        if (b0 >= mis && b0 + 4 <= mis + nb) {
-            v = __ldg(wbase + i);
-        } else {
-#pragma unroll
-            for (uint32_t k = 0; k < 4; k++)
-                if (b0 + k >= mis && b0 + k < mis + nb) v |= (uint32_t)__ldg(lo + (b0 + k - mis)) << (8 * k);
-        }
-        s[i] = v;
-    }
-}
-
-// The 31 bytes of row t of a staged tile as 8 little-endian words (byte 31 = the next row's first byte, replaced by the caller)
-__device__ __forceinline__ void row_words(const uint32_t* s, uint32_t mis, uint32_t t, uint32_t (&w)[8]) {
-    const uint32_t sb = mis + t * R_COLS, wi = sb >> 2, sh = (sb & 3u) * 8u;
-#pragma unroll
-    for (int k = 0; k < 8; k++) w[k] = __funnelshift_r(s[wi + k], s[wi + k + 1], sh);
-}
+constexpr int BI_ROWS = 256;                  // rows per block, one per thread
+constexpr int BI_WORDS = tile_words(BI_ROWS);
 
 __global__ void __launch_bounds__(BI_ROWS) k_batch_in(const uint8_t* __restrict__ tok, const uint8_t* __restrict__ qual, uint64_t rows,
                                                      uint8_t* __restrict__ mat_b, uint8_t* __restrict__ mat_q,

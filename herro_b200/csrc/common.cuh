@@ -213,6 +213,14 @@ __device__ __forceinline__ QView make_qview(const ReadStoreView& rs, const DevOv
     return v;
 }
 
+// OrderedFloat's `<` (src/consensus.rs:139): NaN is greatest and equal to itself, -0 == +0.  The argmax over a row of logits
+// that keeps the last maximum (max_by_key) replaces its candidate whenever !of_less(next, candidate).
+__device__ __forceinline__ bool of_less(float a, float b) {
+    if (isnan(a)) return false;
+    if (isnan(b)) return true;
+    return a < b;
+}
+
 __device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(HB_FULL, v, o);

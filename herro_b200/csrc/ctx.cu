@@ -266,6 +266,26 @@ struct hb_ctx {
             if (stream) cudaStreamDestroy(stream);
         }
     } fwd;
+    // hb_consensus_batch's lane, shaped like the forward lane, so that a host can run the consensus of one read while the
+    // forward of the next one runs.  Calls serialise on its mutex.
+    struct ConsLane {
+        std::mutex mu;
+        cudaStream_t stream = nullptr;
+        cudaEvent_t ev[3]{};     // the caller's stream, consensus start, consensus end
+        KTimer kt;
+        PinBuf pin_in, pin_out;  // input region (carve_cons_in); the emitted lengths and bytes
+        DevBuf d_in, d_out;      // input region; the consensus region (carve_cons_out)
+        std::vector<uint32_t> order;       // host scratch: key sorting
+        std::vector<uint8_t> seq;          // the segments before they are copied out
+        std::vector<uint32_t> seg_len;
+        void release() {
+            d_in.release(); d_out.release();
+            pin_in.release(); pin_out.release();
+            for (auto& e : ev) if (e) cudaEventDestroy(e);
+            kt.destroy();
+            if (stream) cudaStreamDestroy(stream);
+        }
+    } cons;
 
     std::deque<Result> results;
     hb_stats stats{};
@@ -759,6 +779,27 @@ int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs&
 
 static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
+// The segments of one read from its windows' emitted bytes, which lie back to back at `bytes` (src/consensus.rs:90-111,222-226):
+// the windows with n_alns >= 2 are concatenated, any other window ends the current segment, and an empty segment is never
+// emitted.  (Trimming the read to its first and last window with n_alns >= 2 changes nothing here: the windows outside that
+// range only end an empty segment.)  Appends to seq / seg_len; returns the bytes consumed.
+uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw, const uint8_t* bytes, std::vector<uint8_t>& seq,
+                         std::vector<uint32_t>& seg_len) {
+    uint64_t o = 0;
+    size_t start = seq.size();
+    for (size_t w = 0; w < nw; w++) {
+        if (nsel[w] >= 2) {
+            seq.insert(seq.end(), bytes + o, bytes + o + outlen[w]);
+        } else if (seq.size() > start) {
+            seg_len.push_back((uint32_t)(seq.size() - start));
+            start = seq.size();
+        }
+        o += outlen[w];
+    }
+    if (seq.size() > start) seg_len.push_back((uint32_t)(seq.size() - start));
+    return o;
+}
+
 int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     if (hbt.tgt.empty()) return HB_OK;
     const double t_begin = now_ms();
@@ -869,17 +910,8 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
             r.status = HB_ERR_CAPACITY;
             r.msg = "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window";
         }
-        std::vector<uint8_t> cur;
+        o += append_segments(h.nsel + tg.win_begin, h.outlen + tg.win_begin, tg.win_end - tg.win_begin, outb + o, r.seq, r.seg_len);
         for (uint32_t w = tg.win_begin; w < tg.win_end; w++) {
-            const uint32_t len = h.outlen[w];
-            if (h.nsel[w] >= 2) {
-                cur.insert(cur.end(), outb + o, outb + o + len);
-            } else if (!cur.empty()) {
-                r.seg_len.push_back((uint32_t)cur.size());
-                r.seq.insert(r.seq.end(), cur.begin(), cur.end());
-                cur.clear();
-            }
-            o += len;
             // algorithmic bytes of the pileup build for this window (SURVEY.md §8d closed form over the
             // 31 columns the kernel consumes)
             const DevWin& dw = hbt.win[w];
@@ -891,10 +923,6 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
                 else cb += (uint64_t)ov.cig_len * W / std::max<uint32_t>(ov.tend - ov.tstart, W);  // device-windowed: its share of the CIGAR
             }
             algo += (uint64_t)(h.nsel[w] + 1) * ((dw.len + 3) / 4 + dw.len) + cb + 2ull * R_COLS * h.L[w];
-        }
-        if (!cur.empty()) {
-            r.seg_len.push_back((uint32_t)cur.size());
-            r.seq.insert(r.seq.end(), cur.begin(), cur.end());
         }
         if (r.status != HB_OK) { r.seg_len.clear(); r.seq.clear(); }
         corrected += r.seq.size();
@@ -1454,6 +1482,203 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     return HB_OK;
 }
 
+// ---------------------------------------------------------------------------------- hb_consensus_batch
+// Its input region: the caller's tokens and logits (host path only: both byte counts are 0 otherwise), the windows' keys, the
+// per-window arrays and the error word.  Carved alike in pinned and in device memory, so one copy moves all of it.
+struct ConsIn {
+    uint8_t* tok;
+    float* logits;
+    uint2* keys;
+    uint32_t *L, *nsel, *nkeys;
+    uint64_t *rowbase, *keybase;
+    unsigned long long* bad;
+};
+size_t carve_cons_in(ConsIn& a, size_t tok_bytes, size_t logit_rows, size_t n_keys, size_t nw, uint8_t* base) {
+    Carve c{base};
+    c(a.tok, tok_bytes);
+    c(a.logits, logit_rows * 5);
+    c(a.keys, std::max<size_t>(n_keys, 1));
+    c(a.L, nw);
+    c(a.nsel, nw);
+    c(a.nkeys, nw);
+    c(a.rowbase, nw);
+    c(a.keybase, nw);
+    c(a.bad, 1);
+    return c.bytes;
+}
+// The consensus region: the rows' emit bytes and the pipeline's consensus arrays (k_cons_count, the scan, k_cons_write)
+size_t carve_cons_out(BatchView& b, size_t rows, size_t nw, uint8_t* base) {
+    Carve c{base};
+    c(b.row_emit, std::max<size_t>(rows, 1));
+    c(b.out_bytes, std::max<size_t>(rows, 1));
+    c(b.w_outlen, nw);
+    c(b.w_outoff, nw);
+    c(b.counters, CNT_N);
+    return c.bytes;
+}
+
+// The work of hb_consensus_batch, with the lane's lock held and the context's device current
+int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, const uint32_t* rows, const uint8_t* n_alns,
+                    const uint8_t* bases, const uint32_t* n_sup, const uint32_t* supported, const float* bases_logits, uint8_t* seqs,
+                    uint32_t* seg_len, uint32_t* n_segs, uint32_t flags, void* stream) {
+    hb_ctx::ConsLane& Cn = ctx->cons;
+    if (!n_windows || !rows || !n_alns || !bases || !n_sup || !supported || !bases_logits || !seqs || !seg_len || !n_segs)
+        return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (flags & ~HB_CONS_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
+    const bool dev = (flags & HB_CONS_DEVICE_PTRS) != 0;
+    {
+        const void* p[10] = {bases, bases_logits, n_windows, rows, n_alns, n_sup, supported, seqs, seg_len, n_segs};
+        static const char* name[10] = {"bases", "bases_logits", "n_windows", "rows", "n_alns", "n_sup", "supported", "seqs", "seg_len", "n_segs"};
+        for (int i = 0; i < 10; i++) {
+            const int k = pointer_kind(p[i], ctx->device);
+            if (dev && i < 2 && k != 1)
+                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is not memory of device " + std::to_string(ctx->device) +
+                                                 " (HB_CONS_DEVICE_PTRS is set)");
+            if ((!dev || i >= 2) && k != 0)
+                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is device memory" + (i < 2 ? " (HB_CONS_DEVICE_PTRS is not set)" : ""));
+        }
+    }
+    // ---- sizes and range checks
+    uint64_t nw = 0;
+    for (uint32_t i = 0; i < n_reads; i++) nw += n_windows[i];
+    if (nw >= (1ull << 31)) return fail(ctx, HB_ERR_CAPACITY, "batch too large: 2^31 windows or more");
+    uint64_t n_rows = 0, n_pos = 0;
+    for (uint64_t w = 0; w < nw; w++) {
+        if (n_alns[w] > TOP_K)
+            return fail(ctx, HB_ERR_ARG, "n_alns[" + std::to_string(w) + "] = " + std::to_string(n_alns[w]) + " is above " + std::to_string(TOP_K));
+        n_rows += rows[w];
+        n_pos += n_sup[w];
+    }
+    for (uint64_t k = 0; k < n_pos; k++)
+        if (supported[2 * k] > 0xffffu || supported[2 * k + 1] > 0xffu)
+            return fail(ctx, HB_ERR_ARG, "supported[" + std::to_string(k) + "] = (" + std::to_string(supported[2 * k]) + ", " +
+                                             std::to_string(supported[2 * k + 1]) + ") is not a (u16 pos, u8 ins) SupportedPos");
+    if (n_pos >= (1ull << 32) || n_rows >= (1ull << 40)) return fail(ctx, HB_ERR_CAPACITY, "batch too large");
+    if (nw == 0) {
+        memset(n_segs, 0, (size_t)n_reads * 4);
+        return HB_OK;
+    }
+    // ---- scratch (grow-only)
+    const size_t tok_bytes = dev ? 0 : (size_t)n_rows * R_COLS, logit_rows = dev ? 0 : (size_t)n_pos;
+    ConsIn hp, dp;
+    const size_t in_sz = carve_cons_in(hp, tok_bytes, logit_rows, n_pos, nw, nullptr);
+    CK(Cn.pin_in.grow(in_sz));
+    carve_cons_in(hp, tok_bytes, logit_rows, n_pos, nw, Cn.pin_in.as<uint8_t>());
+    CK(Cn.d_in.grow(in_sz));
+    carve_cons_in(dp, tok_bytes, logit_rows, n_pos, nw, Cn.d_in.as<uint8_t>());
+    BatchView b{};
+    b.n_win = (uint32_t)nw;
+    b.w_L = dp.L;
+    b.w_nsel = dp.nsel;
+    b.w_rowbase = dp.rowbase;
+    CK(Cn.d_out.grow(carve_cons_out(b, n_rows, nw, nullptr)));
+    carve_cons_out(b, n_rows, nw, Cn.d_out.as<uint8_t>());
+    const size_t out_sz = al256(nw * 4) + n_rows;
+    CK(Cn.pin_out.grow(out_sz));
+    uint32_t* h_outlen = Cn.pin_out.as<uint32_t>();
+    const uint8_t* h_bytes = Cn.pin_out.as<uint8_t>() + al256(nw * 4);
+    // ---- the per-window arrays and the keys: (pos << 8 | ins, logit row) sorted by key, the last of equal keys kept (the
+    // HashMap collect of src/consensus.rs:115-124).  The features stage emits a window's positions in row order, so its keys are
+    // strictly increasing and one pass confirms it; anything else is sorted.
+    uint64_t rb = 0, sb = 0, kb = 0;
+    for (uint64_t w = 0; w < nw; w++) {
+        hp.L[w] = rows[w];
+        hp.nsel[w] = n_alns[w];
+        hp.rowbase[w] = rb;
+        hp.keybase[w] = kb;
+        const uint32_t ns = n_sup[w];
+        const uint32_t* sp = supported + 2 * sb;
+        uint32_t nk = 0;
+        if (n_alns[w] >= 2 && ns) {
+            auto key = [&](uint32_t j) { return sp[2 * j] << 8 | sp[2 * j + 1]; };
+            bool sorted = true;
+            for (uint32_t j = 1; j < ns && sorted; j++) sorted = key(j - 1) < key(j);
+            if (sorted) {
+                for (uint32_t j = 0; j < ns; j++) hp.keys[kb + j] = make_uint2(key(j), (uint32_t)(sb + j));
+                nk = ns;
+            } else {
+                Cn.order.resize(ns);
+                for (uint32_t j = 0; j < ns; j++) Cn.order[j] = j;
+                std::stable_sort(Cn.order.begin(), Cn.order.end(), [&](uint32_t x, uint32_t y) { return key(x) < key(y); });
+                for (uint32_t i = 0; i < ns; i++) {
+                    const uint32_t j = Cn.order[i];
+                    if (i + 1 < ns && key(Cn.order[i + 1]) == key(j)) continue;  // a later duplicate replaces this one
+                    hp.keys[kb + nk++] = make_uint2(key(j), (uint32_t)(sb + j));
+                }
+            }
+        }
+        hp.nkeys[w] = nk;
+        rb += rows[w];
+        sb += ns;
+        kb += nk;
+    }
+    *hp.bad = ~0ull;
+    if (!dev) {
+        memcpy(hp.tok, bases, tok_bytes);
+        memcpy(hp.logits, bases_logits, (size_t)n_pos * 20);
+    }
+    // ---- device work
+    KTimer& kt = Cn.kt;
+    kt.discard();
+    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
+    kt.st = Cn.stream;
+    if (dev) {
+        CK(cudaEventRecord(Cn.ev[0], (cudaStream_t)stream));
+        CK(cudaStreamWaitEvent(Cn.stream, Cn.ev[0], 0));
+    }
+    CK(cudaMemcpyAsync(Cn.d_in.p, Cn.pin_in.p, in_sz, cudaMemcpyHostToDevice, Cn.stream));
+    CK(cudaEventRecord(Cn.ev[1], Cn.stream));
+    const ConsInArgs ca{dev ? bases : dp.tok, dev ? bases_logits : dp.logits, dp.keys, dp.L, dp.nsel, dp.rowbase, dp.keybase, dp.nkeys,
+                        b.row_emit, dp.bad};
+    kt.begin(K_CONSENSUS);
+    launch_cons_in(ca, (uint32_t)nw, Cn.stream);
+    kt.end();
+    const uint64_t launches = 1 + launch_consensus(b, Cn.stream, kt);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(Cn.ev[2], Cn.stream));
+    CK(cudaMemcpyAsync(hp.bad, dp.bad, sizeof(unsigned long long), cudaMemcpyDeviceToHost, Cn.stream));
+    CK(cudaMemcpyAsync(h_outlen, b.w_outlen, nw * 4, cudaMemcpyDeviceToHost, Cn.stream));
+    // the emitted bytes number at most one per row: the row count bounds the copy, as in the pipeline
+    if (n_rows) CK(cudaMemcpyAsync((void*)h_bytes, b.out_bytes, n_rows, cudaMemcpyDeviceToHost, Cn.stream));
+    CK(cudaStreamSynchronize(Cn.stream));
+    if (*hp.bad != ~0ull) {
+        kt.discard();
+        const uint64_t e = *hp.bad, row = e / R_COLS, col = e % R_COLS;
+        const uint64_t w = (uint64_t)(std::upper_bound(hp.rowbase, hp.rowbase + nw, row) - hp.rowbase) - 1;
+        uint64_t r = 0, w0 = 0;
+        while (w0 + n_windows[r] <= w) w0 += n_windows[r++];
+        const uint8_t tok = dev ? 0 : hp.tok[e];
+        return fail(ctx, HB_ERR_INPUT, "consensus() would panic at (read, window, row, column) = (" + std::to_string(r) + ", " +
+                                           std::to_string(w - w0) + ", " + std::to_string(row - hp.rowbase[w]) + ", " + std::to_string(col) +
+                                           (dev ? std::string(")") : "), token " + std::to_string(tok)) +
+                                           (col == 0 ? ": no BASES_UPPER entry for the target column" : ": no BASES_UPPER_COUNTER entry"));
+    }
+    // ---- per-read segments, then the caller's outputs
+    Cn.seq.clear();
+    Cn.seg_len.clear();
+    uint64_t o = 0, w0 = 0;
+    for (uint32_t i = 0; i < n_reads; i++) {
+        const size_t s0 = Cn.seg_len.size();
+        o += append_segments(hp.nsel + w0, h_outlen + w0, n_windows[i], h_bytes + o, Cn.seq, Cn.seg_len);
+        n_segs[i] = (uint32_t)(Cn.seg_len.size() - s0);
+        w0 += n_windows[i];
+    }
+    if (!Cn.seq.empty()) memcpy(seqs, Cn.seq.data(), Cn.seq.size());
+    if (!Cn.seg_len.empty()) memcpy(seg_len, Cn.seg_len.data(), Cn.seg_len.size() * 4);
+    // ---- counters
+    hb_stats S{};
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, Cn.ev[1], Cn.ev[2]));
+    kt.collect(S.ms_kernel, S.n_kernel);
+    kt.on = false;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    hb_stats& T = ctx->stats;
+    T.ms_consensus += ms;
+    T.kernel_launches += launches;
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    return HB_OK;
+}
+
 }  // namespace
 
 // ========================================================================================
@@ -1544,6 +1769,13 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
             if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
         F.d_in.st = F.d_mat.st = F.d_fwd.st = F.stream;
     }
+    {
+        auto& Cn = ctx->cons;
+        if (cudaStreamCreateWithFlags(&Cn.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
+        for (auto& e : Cn.ev)
+            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
+        Cn.d_in.st = Cn.d_out.st = Cn.stream;
+    }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
         cudaMemPool_t pool;
         uint64_t keep = UINT64_MAX;
@@ -1570,11 +1802,13 @@ void hb_destroy(hb_ctx* ctx) {
     cudaSetDevice(ctx->device);
     for (auto& L : ctx->lanes) if (L.stream) cudaStreamSynchronize(L.stream);
     if (ctx->fwd.stream) cudaStreamSynchronize(ctx->fwd.stream);
+    if (ctx->cons.stream) cudaStreamSynchronize(ctx->cons.stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
     DevBuf* bufs[] = {&ctx->d_words, &ctx->d_word_off, &ctx->d_len, &ctx->d_qual, &ctx->d_qual_off, &ctx->d_ln};
     for (DevBuf* b : bufs) b->release();
     for (auto& L : ctx->lanes) L.release();
     ctx->fwd.release();
+    ctx->cons.release();
     ctx->pin_in.release();
     ctx->slots.clear();
     ctx->queue.clear();
@@ -2169,6 +2403,28 @@ int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* base
     t_err_sink = &err;
     int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
     if (rc == HB_OK) rc = forward_batch(ctx, B, Lmax, bases, quals, lens, indices, info_logits, bases_logits, flags, stream);
+    t_err_sink = nullptr;
+    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
+    if (rc != HB_OK) {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        ctx->err = err;
+    }
+    return rc;
+}
+
+int hb_consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, const uint32_t* rows, const uint8_t* n_alns,
+                       const uint8_t* bases, const uint32_t* n_sup, const uint32_t* supported, const float* bases_logits, uint8_t* seqs,
+                       uint32_t* seg_len, uint32_t* n_segs, uint32_t flags, void* stream) {
+    if (!ctx) return HB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->cons.mu);
+    int prev = -1;
+    cudaGetDevice(&prev);
+    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
+    t_err_sink = &err;
+    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
+    if (rc == HB_OK)
+        rc = consensus_batch(ctx, n_reads, n_windows, rows, n_alns, bases, n_sup, supported, bases_logits, seqs, seg_len, n_segs, flags,
+                             stream);
     t_err_sink = nullptr;
     if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
     if (rc != HB_OK) {

@@ -280,12 +280,7 @@ __global__ void __launch_bounds__(128) k_attention(const float* __restrict__ QKV
 }
 
 // ---- heads: base logits (5) + info logit (1), argmax (last maximal index wins, NaN greatest:
-//      Rust max_by_key over OrderedFloat, src/consensus.rs:136-141) written into row_emit. -----
-__device__ __forceinline__ bool of_less(float a, float b) {
-    if (isnan(a)) return false;
-    if (isnan(b)) return true;
-    return a < b;
-}
+//      Rust max_by_key over OrderedFloat, src/consensus.rs:136-141; of_less in common.cuh) written into row_emit. -----
 __global__ void k_heads(BatchView b, FwdWeights wt, uint32_t n0, uint32_t npos, const float* __restrict__ Z,
                         float* __restrict__ logits, float* __restrict__ info) {
     const uint32_t n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;

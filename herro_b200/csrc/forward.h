@@ -177,6 +177,23 @@ void forward_class_flops_per_pos(const FwdWeights& wt, uint64_t (&out)[16]);
 void launch_batch_in(const uint8_t* tok, const uint8_t* qual, uint64_t rows, uint8_t* mat_b, uint8_t* mat_q, unsigned long long* bad,
                      cudaStream_t st);
 
+// cons_in.cu: a caller's ConsensusWindows -> row_emit (class 0..4 | 0x80 if supported) of every row of the windows with
+// n_alns >= 2, at w_rowbase; the smallest linear byte index of a token the reference's consensus() would panic on is atomicMin'ed
+// into *bad
+struct ConsInArgs {
+    const uint8_t* tok;          // [rows][31] BASES_MAP tokens, window after window, any alignment
+    const float* logits;         // [supported][5]
+    const uint2* keys;           // per window from w_keybase: (pos << 8 | ins, logit row), sorted by key, unique
+    const uint32_t* w_L;         // rows
+    const uint32_t* w_nsel;      // n_alns
+    const uint64_t* w_rowbase;   // first row
+    const uint64_t* w_keybase;   // first key
+    const uint32_t* w_nkeys;
+    uint8_t* row_emit;
+    unsigned long long* bad;
+};
+void launch_cons_in(const ConsInArgs& a, uint32_t n_win, cudaStream_t st);
+
 // features.cu
 cudaError_t features_configure(uint32_t W);
 int launch_features_a(const BatchView& b, cudaStream_t st, KTimer& kt);

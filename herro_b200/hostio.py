@@ -231,6 +231,58 @@ def read_feature_batches(read_dir: str, batch_size: int):
     return out
 
 
+@dataclass
+class ConsensusWindow:
+    """What consensus() reads of a ConsensusWindow (src/consensus.rs:22-33)."""
+    wid: int
+    n_alns: int
+    bases: np.ndarray         # [L, 31] u8 tokens
+    supported: np.ndarray     # [n, 2] u32 (pos, ins)
+    bases_logits: np.ndarray  # [n, 5] f32
+
+
+def read_consensus_windows(features_read_dir: str, logits_read_dir: str):
+    """A read's ConsensusWindows in wid order, rebuilt from a `herro features` read directory (tokens from plane 0 through BASES_MAP,
+    n_alns = min(lines of <wid>.ids.txt, 30) as src/features.rs:877 sets it, (pos, ins) from <wid>.supported.npy) and the `predict`
+    output of the same read (<wid>.bases_logits.npy, required exactly for the windows with supported positions).  The wids must be
+    0 .. n-1: consensus_worker waits for all n_total_wins windows of a read (src/consensus.rs:249)."""
+    wids = sorted(int(f[:-len(".features.npy")]) for f in os.listdir(features_read_dir) if f.endswith(".features.npy"))
+    missing = sorted(set(range(len(wids))) - set(wids))
+    if missing or (wids and wids[-1] != len(wids) - 1):
+        gap = missing[0] if missing else len(wids)
+        raise ValueError(f"{features_read_dir}: window {gap} is missing (the windows must be 0 .. n-1; found {len(wids)} up to {wids[-1]})")
+    out = []
+    for wid in wids:
+        feats = np.load(os.path.join(features_read_dir, f"{wid}.features.npy"))
+        if feats.ndim != 3 or feats.shape[0] != 2 or feats.shape[2] != 31:
+            raise ValueError(f"{features_read_dir}/{wid}.features.npy: expected [2, L, 31], got {feats.shape}")
+        sup = np.load(os.path.join(features_read_dir, f"{wid}.supported.npy"))
+        with open(os.path.join(features_read_dir, f"{wid}.ids.txt"), "rb") as f:
+            n_ids = sum(1 for line in f if line.strip())
+        supported = np.stack([sup["pos"].astype(np.uint32), sup["ins"].astype(np.uint32)], axis=1) if len(sup) else np.zeros((0, 2), np.uint32)
+        if len(sup):
+            p = os.path.join(logits_read_dir, f"{wid}.bases_logits.npy")
+            if not os.path.exists(p):
+                raise ValueError(f"{p} is missing: window {wid} has {len(sup)} supported positions")
+            bl = np.load(p)
+            if bl.shape != (len(sup), 5):
+                raise ValueError(f"{p}: expected [{len(sup)}, 5], got {bl.shape}")
+            bl = np.ascontiguousarray(bl, dtype=np.float32)
+        else:
+            bl = np.zeros((0, 5), np.float32)
+        out.append(ConsensusWindow(wid, min(n_ids, 30), BASES_MAP[feats[0]], np.ascontiguousarray(supported), bl))
+    return out
+
+
+def consensus_args(reads):
+    """The arguments of Context.consensus_batch for several reads, each a list of ConsensusWindow in wid order."""
+    wins = [w for r in reads for w in r]
+    bases = np.concatenate([w.bases for w in wins]) if wins else np.zeros((0, 31), np.uint8)
+    bl = np.concatenate([w.bases_logits for w in wins]) if wins else np.zeros((0, 5), np.float32)
+    return ([len(r) for r in reads], [w.bases.shape[0] for w in wins], [w.n_alns for w in wins], np.ascontiguousarray(bases),
+            [w.supported for w in wins], np.ascontiguousarray(bl, dtype=np.float32))
+
+
 def feature_reads(features_dir: str):
     """The read directories of a `herro features` output directory (those holding window files), sorted by name."""
     return [os.path.join(features_dir, d) for d in sorted(os.listdir(features_dir))

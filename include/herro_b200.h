@@ -10,6 +10,7 @@
  *   inference::inference_worker     src/inference.rs:177-212  (spawned at src/lib.rs:189-196)
  *   consensus::consensus_worker     src/consensus.rs:229-263  (spawned at src/lib.rs:198-199)
  *
+ * (all three at once through hb_submit_*; the model call and consensus also one at a time: hb_forward_batch, hb_consensus_batch)
  * with calls into this library (INTEGRATION.md shows the Rust side).  Plain pointers and
  * sizes only; no torch types; never unwinds or aborts (the reference is `panic = "abort"`,
  * Cargo.toml:14-16): every entry point returns HB_OK or a negative hb_status, and
@@ -159,6 +160,64 @@ int hb_submit_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint3
  * corrected_bases are untouched. */
 int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
                      const int32_t* indices, float* info_logits, float* bases_logits, uint32_t flags, void* stream);
+
+/* ---- consensus alone --------------------------------------------------------------------- */
+#define HB_CONS_DEVICE_PTRS 1u /* bases and bases_logits are device pointers on the context's device */
+/* The replacement of consensus() (src/consensus.rs:86-227) on the windows of n_reads reads, for a host that keeps its own features
+ * stage and model call: what consensus_worker does once a read's windows are complete and sorted by wid (src/consensus.rs:246-253).
+ * With W = sum n_windows, N = sum rows and S = sum n_sup:
+ *
+ *   n_windows     [n_reads] host: every window of each read (n_total_wins), 0 allowed
+ *   rows          [W] host: L' of each window (the rows of ConsensusWindow.bases), 0 allowed
+ *   n_alns        [W] host: at most 30
+ *   bases         [N][31] u8: BASES_MAP tokens (src/inference.rs:23-31), window after window, at any alignment
+ *   n_sup         [W] host: supported positions of each window
+ *   supported     [S][2] u32 host: (pos, ins) of each supported position (pos <= 65535, ins <= 255), window after window
+ *   bases_logits  [S][5] f32: one row per supported entry, in the same order (hb_forward_batch returns them so); info logits are
+ *                 not taken, consensus never reads them
+ *   seqs          host, room for N bytes: the segments, read after read, as ASCII ACGT
+ *   seg_len       host, room for W entries: the segment lengths, read after read
+ *   n_segs        [n_reads] host: segments of each read; 0 = no record (consensus() returned None or nothing), as hb_poll_corrected
+ *   stream        with HB_CONS_DEVICE_PTRS: the cudaStream_t whose pending work produces bases / bases_logits (NULL: legacy default)
+ *
+ * What it computes, with the reference's rules where they depart from the obvious:
+ *   - Only the windows from a read's first to its last with n_alns > 1 are kept; one inside that range with n_alns < 2 ends the
+ *     current segment.  Empty segments are never emitted.
+ *   - Row keys: pos starts at -1 and increments on every row whose column 0 is not '*' (token 4); ins counts consecutive '*' rows
+ *     and resets to 0 on any other row.  The key is (pos as u16, ins as u8) with wrap-around, so leading '*' rows have pos 65535 and
+ *     a run of 256 '*' rows wraps ins to 0.  Such windows are taken as they are.
+ *   - The supported entries of a window are collected into a map in order: a later duplicate (pos, ins) replaces an earlier one;
+ *     an entry that matches no row is ignored; rows that share a key after a wrap all use its entry.
+ *   - A supported row emits the argmax of its 5 logits under OrderedFloat: the last maximum wins, NaN is greatest, -0 == +0.
+ *     Class 4 ('*') emits nothing.
+ *   - Any other row votes over columns [0, n_alns]: token 10 ('.') is skipped, the rest counted by BASES_UPPER_COUNTER; the two
+ *     largest counts are taken by a stable descending sort (ties go A < C < G < T < '*'); with tbase = BASES_UPPER[column 0] the row
+ *     emits tbase if the largest count is below 2, or if the two are equal and tbase is one of them, and the largest's base
+ *     otherwise.  '*' emits nothing.
+ *   Columns past n_alns are never read, nor are windows with n_alns < 2.
+ *
+ * Synchronous: returns when the outputs are written.  With HB_CONS_DEVICE_PTRS the library's stream first waits, through an event,
+ * for the work already enqueued on `stream`.  Scratch only grows, so repeated calls of the same or a smaller shape allocate nothing.
+ * It needs no hb_upload_reads and no model call.
+ *
+ * Errors (nothing is written to the outputs; the context stays usable):
+ *   HB_ERR_ARG       a NULL pointer, n_alns above 30, a supported pos above 65535 or ins above 255, or a pointer that does not
+ *                    match the flag (as hb_forward_batch checks it)
+ *   HB_ERR_INPUT     exactly where consensus() would panic: in a voting row of a window with n_alns >= 2, a token >= 11 in a counted
+ *                    column (BASES_UPPER_COUNTER) or token 10 in column 0 (BASES_UPPER).  The message names the first such
+ *                    (read, window, row, column) in row-major order.  The same bytes in a supported row, a column past n_alns or a
+ *                    window with n_alns < 2 are fine.
+ *   HB_ERR_CAPACITY  a batch too large for the scratch or its indexing (2^31 windows, 2^32 supported entries)
+ *   HB_ERR_CUDA      a CUDA failure
+ *
+ * Threading: may be called from any thread, concurrently with hb_submit_*, hb_flush, hb_poll_corrected and hb_forward_batch on the
+ * same context; calls of hb_consensus_batch on one context serialise among themselves.
+ *
+ * Counters: adds to kernel_launches, n_kernel / ms_kernel (HB_K_CONSENSUS; HB_K_SCAN for the scan), ms_consensus and host_allocs
+ * when scratch grows; nothing else. */
+int hb_consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, const uint32_t* rows, const uint8_t* n_alns,
+                       const uint8_t* bases, const uint32_t* n_sup, const uint32_t* supported, const float* bases_logits, uint8_t* seqs,
+                       uint32_t* seg_len, uint32_t* n_segs, uint32_t flags, void* stream);
 
 /* Host-only utility: the windows [*first_window, *end_window) one alignment contributes OverlapWindows to — the
  * coordinate-only part of extract_windows (src/windowing.rs:53-125,260-272).  HB_ERR_INPUT where the reference panics. */
