@@ -21,6 +21,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libherro_b200.so")
 
 HB_FLAG_KEEP_DEBUG = 1
+HB_FLAG_NO_MODEL = 2
 
 OVERLAP_DTYPE = np.dtype(
     {"names": ["qid", "qlen", "qstart", "qend", "strand", "tid", "tlen", "tstart", "tend", "cigar", "cigar_len"],
@@ -51,6 +52,19 @@ class HbStats(C.Structure):
                [("ms_worker_busy", C.c_double), ("ms_worker_gpu_wait", C.c_double)] + \
                [("host_allocs", C.c_uint64), ("ms_host_alloc", C.c_double), ("ms_submit_wait", C.c_double),
                 ("class_flops", C.c_uint64 * 16), ("ms_worker_phase", C.c_double * 8)]
+
+
+class HbFeaturesShape(C.Structure):
+    _fields_ = [("ticket", C.c_uint64)] + [(n, C.c_uint32) for n in ("n_targets", "n_windows", "n_batches", "n_failed")] + \
+               [(n, C.c_uint64) for n in ("n_rows", "n_sup", "n_ids", "n_batch_rows")]
+
+
+FEATURES_OUT_FIELDS = ("status", "n_windows", "rows", "n_alns", "n_sup", "n_ids", "bases", "quals", "supported", "indices", "ids",
+                       "batch_B", "batch_Lmax", "batch_win", "batch_bases", "batch_quals")
+
+
+class HbFeaturesOut(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32)] + [(n, C.c_void_p) for n in FEATURES_OUT_FIELDS]
 
 
 HOST_LIB_PATH = os.path.join(_HERE, "libherro_host.so")
@@ -105,6 +119,8 @@ def load_library():
     L.hb_selftest_pos_attention.argtypes = [C.c_int, u32p, u32, u32, u32, fp, fp, fp]
     L.hb_forward_batch.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp, vp, u32, vp]
     L.hb_consensus_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u32, vp]
+    L.hb_features_batch.argtypes = [vp, u32, vp, vp, vp, C.POINTER(HbFeaturesShape)]
+    L.hb_features_fetch.argtypes = [vp, C.POINTER(HbFeaturesShape), C.POINTER(HbFeaturesOut), u32, vp]
     _lib = L
     return L
 
@@ -112,9 +128,11 @@ def load_library():
 EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "hb_bind_calling_thread", "hb_set_launch_targets", "hb_set_kernel_timing", "hb_extract_windows", "hb_create", "hb_destroy", "hb_upload_reads", "hb_submit_target", "hb_submit_alignments", "hb_flush",
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
-                    "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch"]
+                    "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch",
+                    "hb_features_batch", "hb_features_fetch"]
 HB_FWD_DEVICE_PTRS = 1
 HB_CONS_DEVICE_PTRS = 1
+HB_FEAT_DEVICE_PTRS = 1
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
@@ -211,19 +229,95 @@ class Corrected:
     segments: list  # list[bytes]; empty = read omitted from the output (consensus() returned None)
 
 
+def _split(a, counts):
+    """a split into consecutive pieces of counts[i] entries (numpy arrays or torch tensors)."""
+    counts = [int(c) for c in counts]
+    if type(a).__module__.split(".")[0] == "torch":
+        import torch
+        return list(torch.split(a[:sum(counts)], counts)) if counts else []
+    return np.split(a[:sum(counts)], np.cumsum(counts)[:-1]) if counts else []
+
+
+class Features:
+    """What one Context.features_batch produced (hb_features_batch): the targets in the order given, each with all of its windows
+    in wid order.  Per target: rids, status (0, or the HB_ERR_* code of a target that failed alone), n_windows.  Per window:
+    rows (L'), n_alns, n_sup, n_ids.  Flat, window after window: bases / quals [sum rows, 31] u8, supported [sum n_sup, 2] u32
+    (pos, ins), indices [sum n_sup] i32 (the row of each supported entry), ids [sum n_ids] u32 (query read ids in final rank
+    order).  With batches: batch_B, batch_Lmax, batch_win (the window of each batch slot) and batch_bases / batch_quals
+    [sum B * Lmax, 31] u8, the reference batches padded with 11 / 126.  The bulk arrays are torch CUDA tensors with device=True."""
+
+    def __init__(self, rids, arrays: dict, batch_size: int):
+        self.rids = rids
+        self.batch_size = batch_size
+        self.__dict__.update(arrays)
+        self.win_off = np.zeros(len(self.rids) + 1, np.int64)
+        self.win_off[1:] = np.cumsum(self.n_windows)
+        self.row_off = np.zeros(len(self.rows) + 1, np.int64)
+        self.row_off[1:] = np.cumsum(self.rows)
+        self.sup_off = np.zeros(len(self.rows) + 1, np.int64)
+        self.sup_off[1:] = np.cumsum(self.n_sup)
+        self.id_off = np.zeros(len(self.rows) + 1, np.int64)
+        self.id_off[1:] = np.cumsum(self.n_ids)
+
+    def window(self, w: int) -> dict:
+        """Window w of the window order: L, n_alns, bases, quals, supported, sup_rows and ids, the fields of debug_window."""
+        r0, r1, s0, s1 = self.row_off[w], self.row_off[w + 1], self.sup_off[w], self.sup_off[w + 1]
+        return dict(L=int(self.rows[w]), n_alns=int(self.n_alns[w]), bases=self.bases[r0:r1], quals=self.quals[r0:r1],
+                    supported=self.supported[s0:s1], sup_rows=self.indices[s0:s1], ids=self.ids[self.id_off[w]:self.id_off[w + 1]])
+
+    def batches(self):
+        """Yields the reference batches in order as (windows, bases [B, Lmax, 31], quals [B, Lmax, 31], lens [B] i32, indices: B arrays
+        of i32 rows): the arguments of Context.forward_batch, or of a TorchScript module after the conversion inference() makes.
+        `windows` are the batch's windows as indices into the window order."""
+        if not hasattr(self, "batch_B"):
+            raise ValueError("features_batch(..., batches=True) collates the reference batches")
+        r = s = 0
+        for B, lmax in zip(self.batch_B, self.batch_Lmax):
+            B, lmax = int(B), int(lmax)
+            wins = [int(w) for w in self.batch_win[s:s + B]]
+            n = B * lmax
+            bases = self.batch_bases[r:r + n].reshape(B, lmax, 31)
+            quals = self.batch_quals[r:r + n].reshape(B, lmax, 31)
+            lens = np.array([int(self.n_sup[w]) for w in wins], np.int32)
+            yield wins, bases, quals, lens, [self.indices[self.sup_off[w]:self.sup_off[w + 1]] for w in wins]
+            r += n
+            s += B
+
+    def consensus_args(self, bases_logits):
+        """The arguments of Context.consensus_batch for these targets.  bases_logits: one [n_sup, 5] row per supported entry in the
+        window order - an [S, 5] array or tensor, or, as the model returns them, a list with the logits of each batch of batches()
+        (each [sum lens, 5], or a list of B per-window pieces): the batches hold every window with supported positions once, in the
+        window order."""
+        if isinstance(bases_logits, (list, tuple)):
+            flat = []
+            for x in bases_logits:
+                flat.extend(x if isinstance(x, (list, tuple)) else [x])
+            if type(flat[0] if flat else self.bases).__module__.split(".")[0] == "torch":
+                import torch
+                bases_logits = (torch.cat([x.reshape(-1, 5) for x in flat]).float().contiguous() if flat else
+                                torch.zeros((0, 5), dtype=torch.float32, device=self.bases.device))
+            else:
+                bases_logits = np.ascontiguousarray(np.concatenate([np.asarray(x).reshape(-1, 5) for x in flat]) if flat else
+                                                    np.zeros((0, 5)), dtype=np.float32)
+        return (self.n_windows, self.rows, self.n_alns, self.bases, _split(self.supported, self.n_sup), bases_logits)
+
+
 class Context:
     """One per GPU — the per-device worker group of src/lib.rs:154-200."""
 
-    def __init__(self, model_path: str, device: int = 0, window_size: int = 4096, batch_size: int = 64,
+    def __init__(self, model_path, device: int = 0, window_size: int = 4096, batch_size: int = 64,
                  launch_targets: int = 0, keep_debug: bool = False):
+        """model_path None: a context without weights (HB_FLAG_NO_MODEL), for features_batch and consensus_batch around a model
+        the caller runs itself."""
         self._L = load_library()
         self._h = C.c_void_p()
         opt = HbOptions(C.sizeof(HbOptions), window_size, batch_size, launch_targets,
-                        HB_FLAG_KEEP_DEBUG if keep_debug else 0)
-        rc = self._L.hb_create(C.byref(self._h), device, model_path.encode(), C.byref(opt))
+                        (HB_FLAG_KEEP_DEBUG if keep_debug else 0) | (HB_FLAG_NO_MODEL if model_path is None else 0))
+        rc = self._L.hb_create(C.byref(self._h), device, None if model_path is None else model_path.encode(), C.byref(opt))
         if rc != 0:
             raise HerroError(rc, self._L.hb_last_error(None).decode())
         self.window_size = window_size
+        self.batch_size = batch_size
         self.device = device
         self._keep = []
         self.read_len = None
@@ -419,6 +513,70 @@ class Context:
                 s += 1
             out.append(segs)
         return out
+
+    # -- the features stage alone -------------------------------------------------------
+    def features_batch(self, targets, device: bool = False, batches: bool = False) -> Features:
+        """extract_features (src/features.rs:326-583) on many targets (hb_features_batch + hb_features_fetch): targets is a list of
+        (rid, overlaps), overlaps as make_overlaps builds them (`(tid, Vec<Alignment>)`).  device: the bulk arrays (bases, quals,
+        batch_bases, batch_quals) become torch.uint8 tensors on the context's device, written on torch's current stream; batches:
+        also collate the reference batches of `-b` (batch_size) windows.  -> Features."""
+        if not isinstance(device, bool) or not isinstance(batches, bool):
+            raise TypeError("device and batches must be bools")
+        targets = list(targets)
+        rids = np.zeros(len(targets), np.uint32)
+        ovs = []
+        for k, t in enumerate(targets):
+            if not isinstance(t, (tuple, list)) or len(t) != 2:
+                raise TypeError(f"targets[{k}] must be a (rid, overlaps) pair")
+            rid, o = t
+            if isinstance(rid, (bool, np.bool_)) or not isinstance(rid, (int, np.integer)) or not 0 <= int(rid) < 2 ** 32:
+                raise ValueError(f"targets[{k}]: rid must be an integer in [0, 2^32), got {rid!r}")
+            if not isinstance(o, np.ndarray) or o.dtype != OVERLAP_DTYPE or o.ndim != 1:
+                raise TypeError(f"targets[{k}]: overlaps must be a 1-D OVERLAP_DTYPE array (Context.make_overlaps)")
+            rids[k] = int(rid)
+            ovs.append(o)
+        n_ovl = np.array([len(o) for o in ovs], np.uint32)
+        ovl = np.zeros(int(n_ovl.sum()), OVERLAP_DTYPE)  # not np.concatenate: its dtype promotion packs the padded hb_overlap layout
+        o0 = 0
+        for o in ovs:
+            ovl[o0:o0 + len(o)] = o
+            o0 += len(o)
+        L = self._L
+        sh = HbFeaturesShape()
+        self._check(L.hb_features_batch(self._h, len(rids), rids.ctypes.data, n_ovl.ctypes.data, ovl.ctypes.data if len(ovl) else None,
+                                        C.byref(sh)))
+        nt, nw, nb, N, S, NI, NB = sh.n_targets, sh.n_windows, sh.n_batches, sh.n_rows, sh.n_sup, sh.n_ids, sh.n_batch_rows
+        a = dict(status=np.zeros(max(nt, 1), np.int32), n_windows=np.zeros(max(nt, 1), np.uint32), rows=np.zeros(max(nw, 1), np.uint32),
+                 n_alns=np.zeros(max(nw, 1), np.uint8), n_sup=np.zeros(max(nw, 1), np.uint32), n_ids=np.zeros(max(nw, 1), np.uint32),
+                 supported=np.zeros((max(S, 1), 2), np.uint32), indices=np.zeros(max(S, 1), np.int32), ids=np.zeros(max(NI, 1), np.uint32))
+        if device:
+            import torch
+            dev = torch.device("cuda", self.device)
+            bulk = lambda n: torch.empty((max(n, 1), 31), dtype=torch.uint8, device=dev)  # noqa: E731
+        else:
+            bulk = lambda n: np.empty((max(n, 1), 31), np.uint8)  # noqa: E731
+        a["bases"], a["quals"] = bulk(N), bulk(N)
+        if batches:
+            nslots = 0  # sum B, known once batch_B is fetched
+            a["batch_B"], a["batch_Lmax"] = np.zeros(max(nb, 1), np.uint32), np.zeros(max(nb, 1), np.uint32)
+            a["batch_bases"], a["batch_quals"] = bulk(NB), bulk(NB)
+            o = HbFeaturesOut(C.sizeof(HbFeaturesOut))
+            o.batch_B = a["batch_B"].ctypes.data
+            self._check(L.hb_features_fetch(self._h, C.byref(sh), C.byref(o), 0, None))
+            nslots = int(a["batch_B"][:nb].sum())
+            a["batch_win"] = np.zeros(max(nslots, 1), np.uint32)
+        o = HbFeaturesOut(C.sizeof(HbFeaturesOut))
+        for name, x in a.items():
+            setattr(o, name, x.data_ptr() if device and name in ("bases", "quals", "batch_bases", "batch_quals") else x.ctypes.data)
+        stream = torch.cuda.current_stream(dev).cuda_stream if device else None
+        self._check(L.hb_features_fetch(self._h, C.byref(sh), C.byref(o), HB_FEAT_DEVICE_PTRS if device else 0, stream))
+        size = dict(status=nt, n_windows=nt, rows=nw, n_alns=nw, n_sup=nw, n_ids=nw, bases=N, quals=N, supported=S, indices=S, ids=NI,
+                    batch_B=nb, batch_Lmax=nb, batch_bases=NB, batch_quals=NB)
+        if batches:
+            size["batch_win"] = nslots
+        a = {k: v[:size[k]] for k, v in a.items()}
+        self.last_features_shape = sh
+        return Features([int(r) for r in rids], a, self.batch_size)
 
     def set_launch_targets(self, n: int):
         self._check(self._L.hb_set_launch_targets(self._h, n))

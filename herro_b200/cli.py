@@ -2,13 +2,15 @@
 as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp -> the C ABI of libherro_b200):
 
     python -m herro_b200.cli inference --read-alns <dir> -t 4 -d 0 -m model.hbw -b 64 reads.fastq out.fasta
-    python -m herro_b200.cli features  --read-alns <dir> -m model.hbw reads.fastq out_dir
+    python -m herro_b200.cli inference --torch --read-alns <dir> -d 0 -m model.pt -b 64 reads.fastq out.fasta
+                                       (any TorchScript graph with the reference's forward signature, run by torch.jit)
+    python -m herro_b200.cli features  --read-alns <dir> reads.fastq out_dir
     python -m herro_b200.cli predict   -m model.hbw -b 64 [-d 0] features_dir out_dir   (the model alone, on `features` output)
     python -m herro_b200.cli consensus -m model.hbw [-d 0] features_dir logits_dir reads.fastq out.fasta
                                        (consensus alone, on `features` and `predict` output)
 
 Nothing is computed here: FASTQ parsing / 2-bit packing, `*.oec.zst` decoding and PAF parsing, the feature / consumer threads
-and the FASTA writer are C++ threads (hbh_inference); `features` drives hb_dump_features launch by launch.  In deployment this
+and the FASTA writer are C++ threads (hbh_inference); `features` and `inference --torch` call hb_features_batch.  In deployment this
 role is played by the unchanged Rust binary (INTEGRATION.md); the flags keep the reference's meaning: reads shorter than `-w`
 are not loaded (src/haec_io.rs:48), unknown names / self overlaps / repeated (query,target) pairs are skipped
 (src/overlaps.rs:137-185), `-c` cluster files restrict targets to core reads (:154-159).
@@ -49,25 +51,78 @@ def inference(args):
     return r
 
 
+def write_features(F, k, out_dir, names):
+    """The feature files of target k of a Features result (Context.features_batch) under out_dir/<read name>/."""
+    d = os.path.join(out_dir, os.fsdecode(names[F.rids[k]]))
+    for wid in range(int(F.n_windows[k])):
+        w = F.window(int(F.win_off[k]) + wid)
+        hostio.write_feature_window(d, wid, w["bases"], w["quals"], w["supported"], [names[int(q)] for q in w["ids"]])
+
+
 def features(args):
-    """`herro features` (src/lib.rs:50-111): the per-window feature files of every target, from the device path."""
+    """`herro features` (src/lib.rs:50-111): the per-window feature files of every target, from hb_features_batch on a context
+    without weights, `--targets-per-launch` targets per call."""
     R = hostio.Reads(args.reads, min_len=args.window_size)
     A = hostio.Alignments(args.read_alns, R)
-    ctx = api.Context(args.model, 0, args.window_size, 64, launch_targets=1 << 20, keep_debug=True)
+    ctx = api.Context(None, 0, args.window_size, 64)
     R.upload(ctx)
     n = 0
     step = max(1, args.targets_per_launch)
-    for k0 in range(0, A.n_targets, step):  # the debug taps keep one launch: dump launch by launch
-        group = range(k0, min(k0 + step, A.n_targets))
-        for k in group:
-            rid, ov = A.target(k)
-            ctx.submit_alignments(rid, ov)
-        ctx.flush()
-        ctx.drain(skip_failed=True)
-        for k in group:
-            ctx.dump_features(int(A.target_rids[k]), args.output, R.ids)
+    for k0 in range(0, A.n_targets, step):
+        F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))])
+        for k in range(len(F.rids)):
+            if F.status[k]:  # the reference would have panicked on this read's alignments
+                print(f"skipped read {os.fsdecode(R.ids[F.rids[k]])}: error {int(F.status[k])}", file=sys.stderr)
+                continue
+            write_features(F, k, args.output, R.ids)
             n += 1
+    ctx.close()
     print(f"Wrote the feature files of {n} reads under {args.output}.", file=sys.stderr)
+
+
+def quals_normalised(quals):
+    """inference()'s quality transform (src/inference.rs:19-21,152-153): fp32, multiply then subtract."""
+    import torch
+    return (2.0 / 93.0) * quals.to(torch.float32) - (2.0 * 33.0 / 93.0 + 1.0)
+
+
+def inference_torch(args):
+    """`inference --torch`: the features stage and consensus on the device through the library (a context without weights), the
+    model call by torch.jit on a TorchScript archive the library does not parse, as src/inference.rs:147-175 calls it: int tokens,
+    normalised qualities, lens and the indices list.  One device; `--targets-per-launch` targets per features call."""
+    import numpy as np
+    import torch
+    dev = int(str(args.devices).split(",")[0])
+    if "," in str(args.devices):
+        raise SystemExit("--torch runs on one device (-d)")
+    R = hostio.Reads(args.reads, min_len=args.window_size)
+    A = hostio.Alignments(args.read_alns, R)
+    ctx = api.Context(None, dev, args.window_size, args.batch_size)
+    R.upload(ctx)
+    cuda = torch.device("cuda", dev)
+    module = torch.jit.load(args.model, map_location=cuda).eval()
+    out = hostio.FastaWriter(args.output)
+    step = max(1, args.targets_per_launch)
+    failed = 0
+    with torch.no_grad(), torch.cuda.device(cuda):
+        for k0 in range(0, A.n_targets, step):
+            F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))], device=True, batches=True)
+            logits = []
+            for _, bases, quals, lens, indices in F.batches():
+                idx = [torch.from_numpy(np.ascontiguousarray(i)).to(cuda) for i in indices]
+                _, bl = module(bases.to(torch.int32), quals_normalised(quals), torch.from_numpy(lens).to(cuda), idx)
+                logits.append(bl.float())
+            for k, segs in enumerate(ctx.consensus_batch(*F.consensus_args(logits))):
+                rid = F.rids[k]
+                if F.status[k]:
+                    failed += 1
+                elif segs:
+                    out.write(R.ids[rid], R.descriptions[rid], segs)
+    records, bases = out.close()
+    ctx.close()
+    print(f"Processed {A.n_targets} reads, wrote {records} records ({bases} bases)" + (f"; skipped {failed} reads" if failed else ""),
+          file=sys.stderr)
+    return dict(targets=A.n_targets, records=records, corrected_bases=bases, failed_targets=failed)
 
 
 def predict(args):
@@ -136,13 +191,17 @@ def main(argv=None):
     inf.add_argument("-d", dest="devices", default="0")
     inf.add_argument("-b", dest="batch_size", type=int, required=True)
     inf.add_argument("-c", dest="cluster", default="")
+    inf.add_argument("--torch", action="store_true",
+                     help="-m is a TorchScript archive that torch.jit runs (any graph with the reference's forward signature); features "
+                          "and consensus run in the library")
+    inf.add_argument("--targets-per-launch", type=int, default=256, help="with --torch: targets per features call")
     inf.add_argument("reads")
     inf.add_argument("output")
     ft = sub.add_parser("features")
     ft.add_argument("--read-alns", required=True)
     ft.add_argument("-w", dest="window_size", type=int, default=4096)
-    ft.add_argument("-m", dest="model", required=True, help="weights (a context needs them; the feature files do not depend on them)")
-    ft.add_argument("--targets-per-launch", type=int, default=256)
+    ft.add_argument("-m", dest="model", default=None, help="accepted and ignored: the feature files do not depend on the model")
+    ft.add_argument("--targets-per-launch", type=int, default=256, help="targets per features call")
     ft.add_argument("reads")
     ft.add_argument("output")
     pr = sub.add_parser("predict", help="the model alone on a `features` output directory")
@@ -161,6 +220,10 @@ def main(argv=None):
     cs.add_argument("output")
     args = ap.parse_args(argv)
     if args.cmd == "inference":
+        if args.torch:
+            if args.cluster:
+                raise SystemExit("-c is not supported with --torch")
+            return inference_torch(args)
         return inference(args)
     if args.cmd == "predict":
         return predict(args)

@@ -190,6 +190,20 @@ struct LastLaunch {  // host copies of per-window metadata of the most recent la
     FwdBufs fwd;
 };
 
+// What one hb_features_batch produced, in the caller's order (targets as given, each target's windows in wid order).  The bulk
+// arrays stay in the features lane's regions until hb_features_fetch copies them out.
+struct FeatResult {
+    bool valid = false;
+    hb_features_shape shape{};
+    BatchView view;                       // the lane's regions as the call left them
+    std::vector<int32_t> status;          // per target
+    std::vector<uint32_t> n_windows;
+    std::vector<uint32_t> rows, n_sup, n_ids, dev_win;  // per window; dev_win: the window in `view`, ~0u for a failed target
+    std::vector<uint8_t> n_alns;
+    std::vector<uint64_t> dev_rowbase;    // per window of `view`: its first row in the row arena
+    std::vector<uint32_t> batch_B, batch_Lmax, batch_win;
+};
+
 }  // namespace
 
 struct hb_ctx {
@@ -286,6 +300,25 @@ struct hb_ctx {
             if (stream) cudaStreamDestroy(stream);
         }
     } cons;
+    // hb_features_batch's lane: a launch lane that no worker owns (stream, events, timer, batch and row regions) and never publishes
+    // its sizes to the pipeline's lanes, its own staging batch, and the tables and staging of hb_features_fetch.  Calls of
+    // hb_features_batch and hb_features_fetch serialise on its mutex.
+    struct FeatLane {
+        std::mutex mu;
+        Lane lane;
+        HostBatch hbt;
+        PinBuf pin_n1, pin_tab;  // the windows' surviving-overlap counts; the output tables, staged for one copy
+        DevBuf d_tab, d_out;     // the output tables; the host-bound outputs before their copy
+        FeatResult res;
+        uint64_t ticket = 0;
+        void release() {
+            lane.release();
+            pin_n1.release(); pin_tab.release();
+            d_tab.release(); d_out.release();
+            hbt = HostBatch();
+        }
+    } feat;
+    bool no_model = false;  // HB_FLAG_NO_MODEL: no weights; the calls that run the forward refuse
 
     std::deque<Result> results;
     hb_stats stats{};
@@ -800,22 +833,21 @@ uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw
     return o;
 }
 
-int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
-    if (hbt.tgt.empty()) return HB_OK;
-    const double t_begin = now_ms();
-    double t_wait = 0, t_mark = t_begin;
-    hb_stats S{};  // merged into ctx->stats under the lock at the end
 #define SYNC_TIMED() do { const double t__ = now_ms(); CK(cudaStreamSynchronize(L->stream)); t_wait += now_ms() - t__; } while (0)
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
-    std::vector<Result> out_results;
+
+// The front half of a launch, shared by run_batch and hb_features_batch: carve the batch region for the staged batch, copy it in,
+// and run windowing, the pileup and the per-window lists until the row arena holds every row (it is regrown on overflow).  On
+// return `b` views the lane's regions, h.cnt / h.nsup hold the counts of the last attempt, ev[0] / ev[2] bracket its feature
+// kernels, and *total_rows is the rows of all windows.
+int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, Readback& h, uint64_t* launches, uint64_t* total_rows,
+              hb_stats& S, double& t_wait, double& t_mark) {
     const uint32_t W = ctx->opt.window_size;
     const size_t nt = hbt.tgt.size(), nw = hbt.win.size();
-    // the regions may move below: the view kept from the lane's previous launch would point into freed memory
-    L->last.valid = false;
     const size_t cig_bytes = hbt.cig.size();
     const uint64_t op_slots = hbt.op_cap + hbt.dev_op_cap, raw_slots = hbt.raw_cap;
     if (op_slots >= 0xffffffffull) return fail(ctx, HB_ERR_CAPACITY, "batch too large: more than 2^32 CIGAR ops (lower launch_targets)");
-    BatchView b = make_view(ctx, hbt);
+    b = make_view(ctx, hbt);
     CK(L->d_batch.grow(carve_batch(b, cig_bytes, op_slots, raw_slots, nullptr)));
     carve_batch(b, cig_bytes, op_slots, raw_slots, L->d_batch.as<uint8_t>());
     // ---- H2D straight from the pinned staging arrays of the batch
@@ -830,11 +862,8 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     const uint64_t per_win = ctx->arena_rows_per_win ? ctx->arena_rows_per_win : (uint64_t)W + W / 2;
     int rc = set_rows(ctx, L, b, L->rows_cap ? L->rows_cap : (uint64_t)nw * per_win + 64);
     if (rc) return rc;
-    Readback h;
     CK(L->pin_small.grow(carve_readback(h, nt, nw, nullptr)));
     carve_readback(h, nt, nw, L->pin_small.as<uint8_t>());
-    uint64_t launches = 0;
-    uint64_t total_rows = 0;
     PHASE(0);
     L->kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
     L->kt.st = L->stream;
@@ -843,22 +872,43 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         rc = zero_scratch(ctx, L, b);
         if (rc) return rc;
         CK(cudaEventRecord(L->ev[0], L->stream));
-        launches += launch_features_a(b, L->stream, L->kt);
+        *launches += launch_features_a(b, L->stream, L->kt);
         CK(cudaEventRecord(L->ev[1], L->stream));
-        launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
+        *launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
         CK(cudaEventRecord(L->ev[2], L->stream));
-        launches += launch_features_c1(b, L->stream, L->kt);  // ref_lmax + scan; the work list needs its buffers first
+        *launches += launch_features_c1(b, L->stream, L->kt);  // ref_lmax + scan; the work list needs its buffers first
         CK(cudaMemcpyAsync(h.cnt, b.counters, CNT_N * 4, cudaMemcpyDeviceToHost, L->stream));
         CK(cudaMemcpyAsync(h.nsup, b.w_nsup, nw * 4, cudaMemcpyDeviceToHost, L->stream));  // the forward passes end at window boundaries
         PHASE(1);
         SYNC_TIMED();
         PHASE(2);
-        total_rows = (uint64_t)h.cnt[CNT_TOTAL_ROWS] | ((uint64_t)h.cnt[CNT_TOTAL_ROWS + 1] << 32);
+        *total_rows = (uint64_t)h.cnt[CNT_TOTAL_ROWS] | ((uint64_t)h.cnt[CNT_TOTAL_ROWS + 1] << 32);
         if (!h.cnt[CNT_OVERFLOW]) break;
         if (attempt >= 2) return fail(ctx, HB_ERR_CAPACITY, "row arena overflow persisted after regrowth");
-        rc = set_rows(ctx, L, b, total_rows + total_rows / 8 + 4096);
+        rc = set_rows(ctx, L, b, *total_rows + *total_rows / 8 + 4096);
         if (rc) return rc;
     }
+    return HB_OK;
+}
+
+int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
+    if (hbt.tgt.empty()) return HB_OK;
+    const double t_begin = now_ms();
+    double t_wait = 0, t_mark = t_begin;
+    hb_stats S{};  // merged into ctx->stats under the lock at the end
+    std::vector<Result> out_results;
+    const uint32_t W = ctx->opt.window_size;
+    const size_t nt = hbt.tgt.size(), nw = hbt.win.size();
+    // the regions may move below: the view kept from the lane's previous launch would point into freed memory
+    L->last.valid = false;
+    const size_t cig_bytes = hbt.cig.size();
+    const uint64_t op_slots = hbt.op_cap + hbt.dev_op_cap, raw_slots = hbt.raw_cap;
+    BatchView b;
+    Readback h;
+    uint64_t launches = 0;
+    uint64_t total_rows = 0;
+    int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, S, t_wait, t_mark);
+    if (rc) return rc;
     const uint64_t n_sup = (uint64_t)h.cnt[CNT_NSUP] | ((uint64_t)h.cnt[CNT_NSUP + 1] << 32);
     const uint32_t max_nsup = nw ? *std::max_element(h.nsup, h.nsup + nw) : 0;
     FwdBufs f;
@@ -1312,6 +1362,63 @@ int stage_target(hb_ctx* ctx, const PreparedTarget& P, const hb_overlap* ovl, ui
     return HB_OK;
 }
 
+// The target preparation of hb_submit_alignments, shared with hb_features_batch: checks the alignments of target `rid` and lays
+// out the target's overlap-windows in P.  HB_ERR_INPUT: coordinates (or, with host windowing, a CIGAR) the reference would panic
+// on; any other error is the caller's.
+int prepare_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_t n_ovl, PreparedTarget& P) {
+    if (!ctx->have_reads) return fail(ctx, HB_ERR_STATE, "hb_upload_reads must be called before submitting targets");
+    if (rid >= ctx->n_reads) return fail(ctx, HB_ERR_ARG, "rid out of range");
+    if (n_ovl && !ovl) return fail(ctx, HB_ERR_ARG, "null array");
+    const uint32_t W = ctx->opt.window_size;
+    const uint32_t n_windows = (ctx->read_len[rid] + W - 1) / W;
+    if (ctx->host_windowing) {  // A-B path: extract_windows on the calling thread, then the hb_submit_target route
+        thread_local std::vector<hb_overlap_window> ows;
+        ows.clear();
+        for (uint32_t i = 0; i < n_ovl; i++) {
+            if (ovl[i].tid != rid) return fail(ctx, HB_ERR_ARG, "overlap.tid != rid");
+            if (host_extract_windows(ovl[i], i, W, n_windows, ows) != 0)
+                return fail(ctx, HB_ERR_INPUT, "malformed alignment (CIGAR / coordinates) for target " + std::to_string(rid));
+        }
+        P.raw = false;
+        return prepare_target(ctx, rid, n_windows, ovl, n_ovl, ows.data(), (uint32_t)ows.size(), P);
+    }
+    // Device windowing (windowing_dev.cu): the host only lays out which (alignment, window) pairs exist — a function of the PAF
+    // coordinates — and ships the CIGARs; a CIGAR that is malformed or disagrees with its coordinates fails this target on the
+    // device (tgt_err) instead of here.
+    thread_local std::vector<uint32_t> first, fill;
+    P.raw = true;
+    P.rid = rid; P.n_windows = n_windows; P.len = ctx->read_len[rid];
+    P.win_begin.assign(n_windows + 1, 0);
+    P.aln_now.assign(n_ovl, 0);
+    first.assign(n_ovl, 0);
+    uint64_t cb = 0;
+    for (uint32_t i = 0; i < n_ovl; i++) {
+        if (ovl[i].tid != rid) return fail(ctx, HB_ERR_ARG, "overlap.tid != rid (alignments must be grouped by target)");
+        if (ovl[i].qid >= ctx->n_reads) return fail(ctx, HB_ERR_ARG, "overlap.qid out of range");
+        if (!ovl[i].cigar && ovl[i].cigar_len) return fail(ctx, HB_ERR_ARG, "null cigar");
+        if (ovl[i].strand > 1) return fail(ctx, HB_ERR_ARG, "strand must be 0 or 1");
+        uint32_t wa, we;
+        if (skeleton_for_alignment(ovl[i], W, n_windows, wa, we) != 0)
+            return fail(ctx, HB_ERR_INPUT, "malformed alignment (coordinates) for target " + std::to_string(rid));
+        first[i] = wa;
+        P.aln_now[i] = we - wa;
+        if (we > wa) cb += ovl[i].cigar_len;
+        for (uint32_t w = wa; w < we; w++) P.win_begin[w + 1]++;
+    }
+    for (uint32_t w = 0; w < n_windows; w++) P.win_begin[w + 1] += P.win_begin[w];
+    P.cig_bytes = cb;
+    P.ow.resize(P.win_begin[n_windows]);
+    fill.assign(P.win_begin.begin(), P.win_begin.end() - 1);
+    for (uint32_t i = 0; i < n_ovl; i++)  // alignment order inside every window = the reference's push order
+        for (uint32_t w = first[i]; w < first[i] + P.aln_now[i]; w++) P.ow[fill[w]++] = DevOW{i, w, 0, 0, 0, 0, 0, 0, 0, 0};
+    return HB_OK;
+}
+
+int no_model_fail(hb_ctx* ctx) {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    return fail(ctx, HB_ERR_STATE, "the context was created with HB_FLAG_NO_MODEL: it has no weights to run the forward with");
+}
+
 // ---------------------------------------------------------------------------------- hb_forward_batch
 // Its input region: the caller's tokens and qualities (host path only: in_bytes is 0 otherwise), the per-window arrays of the
 // view and the error word.  Carved alike in pinned and in device memory, so one copy moves all of it.
@@ -1679,6 +1786,294 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
     return HB_OK;
 }
 
+// ---------------------------------------------------------------------------------- hb_features_batch / hb_features_fetch
+// The work of hb_features_batch, with the lane's lock held and the context's device current
+int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const uint32_t* n_ovl, const hb_overlap* ovl,
+                   hb_features_shape* shape) {
+    hb_ctx::FeatLane& Fl = ctx->feat;
+    FeatResult& R = Fl.res;
+    R.valid = false;  // the regions may move below
+    if (!shape || (n_targets && (!rids || !n_ovl))) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (!ctx->have_reads) return fail(ctx, HB_ERR_STATE, "hb_upload_reads must be called before hb_features_batch");
+    uint64_t n_all = 0;
+    for (uint32_t i = 0; i < n_targets; i++) n_all += n_ovl[i];
+    if (n_all && !ovl) return fail(ctx, HB_ERR_ARG, "null pointer");
+    const uint32_t W = ctx->opt.window_size, bs = ctx->opt.batch_size;
+    // ---- every target prepared as hb_submit_alignments prepares it; coordinates the reference would panic on fail that target alone
+    HostBatch& hbt = Fl.hbt;
+    hbt.clear();
+    R.status.assign(n_targets, HB_OK);
+    R.n_windows.resize(n_targets);
+    thread_local PreparedTarget P;
+    std::string first_err;
+    const hb_overlap* o = ovl;
+    for (uint32_t i = 0; i < n_targets; i++) {
+        const int rc = prepare_alignments(ctx, rids[i], o, n_ovl[i], P);
+        if (rc == HB_ERR_INPUT) {
+            R.status[i] = HB_ERR_INPUT;
+            if (first_err.empty()) first_err = "target " + std::to_string(rids[i]) + ": " + errref(ctx);
+        } else if (rc) {
+            errref(ctx) = "target " + std::to_string(i) + " (rid " + std::to_string(rids[i]) + "): " + errref(ctx);
+            return rc;
+        } else {
+            const int ra = append_target(ctx, hbt, P, o, n_ovl[i]);
+            if (ra) return ra;
+        }
+        R.n_windows[i] = (ctx->read_len[rids[i]] + W - 1) / W;
+        o += n_ovl[i];
+    }
+    // ---- the front half of a launch on the lane
+    hb_ctx::Lane* L = &Fl.lane;
+    const size_t nt = hbt.tgt.size(), nw = hbt.win.size();
+    BatchView b{};
+    Readback h{};
+    uint64_t launches = 0, total_rows = 0;
+    hb_stats S{};
+    double t_wait = 0, t_mark = now_ms();
+    float ms_front = 0;
+    if (nt) {
+        int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, S, t_wait, t_mark);
+        if (rc) { L->kt.discard(); return rc; }
+        CK(Fl.pin_n1.grow(nw * 4));
+        uint32_t* n1 = Fl.pin_n1.as<uint32_t>();
+        CK(cudaMemcpyAsync(h.L, b.w_L, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaMemcpyAsync(h.nsel, b.w_nsel, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaMemcpyAsync(h.terr, b.tgt_err, nt * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaMemcpyAsync(n1, b.w_n1, nw * 4, cudaMemcpyDeviceToHost, L->stream));
+        CK(cudaStreamSynchronize(L->stream));
+        CK(cudaEventElapsedTime(&ms_front, L->ev[0], L->ev[2]));
+        S.h2d_bytes = vbytes(hbt.tgt) + vbytes(hbt.win) + vbytes(hbt.ovl) + vbytes(hbt.ow) + hbt.cig.size();
+        S.d2h_bytes = CNT_N * 4 + nw * 16 + nt * 4;
+        L->kt.collect(S.ms_kernel, S.n_kernel);
+        L->kt.on = false;
+    }
+    // ---- the caller's tables: windows of the targets in the given order, a failed target's without content
+    R.rows.clear(); R.n_alns.clear(); R.n_sup.clear(); R.n_ids.clear(); R.dev_win.clear();
+    R.batch_B.clear(); R.batch_Lmax.clear(); R.batch_win.clear();
+    R.dev_rowbase.resize(nw);
+    uint64_t rb = 0;
+    for (size_t w = 0; w < nw; w++) { R.dev_rowbase[w] = rb; rb += h.L[w]; }
+    hb_features_shape sh{};
+    size_t t_dev = 0;  // the next target of the device batch
+    uint32_t n_failed = 0;
+    const uint32_t* n1 = Fl.pin_n1.as<uint32_t>();
+    for (uint32_t i = 0; i < n_targets; i++) {
+        const uint32_t nwin = R.n_windows[i];
+        const uint32_t w_out0 = (uint32_t)R.rows.size();
+        uint32_t dw0 = ~0u;
+        if (R.status[i] == HB_OK) {
+            const DevTarget& tg = hbt.tgt[t_dev++];
+            if (h.terr[t_dev - 1] & TERR_BAD_INPUT) R.status[i] = HB_ERR_INPUT;
+            else if (h.terr[t_dev - 1] & TERR_TOO_MANY_COLS) R.status[i] = HB_ERR_CAPACITY;
+            if (R.status[i] == HB_OK) dw0 = tg.win_begin;
+            else if (first_err.empty())
+                first_err = "target " + std::to_string(rids[i]) + ": " +
+                            (R.status[i] == HB_ERR_INPUT ? std::string("input the reference would panic on (malformed CIGAR / window descriptor / query coordinates)")
+                                                         : "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window");
+        }
+        if (R.status[i] != HB_OK) n_failed++;
+        for (uint32_t k = 0; k < nwin; k++) {
+            const bool ok = dw0 != ~0u;
+            const uint32_t dw = ok ? dw0 + k : ~0u;
+            R.dev_win.push_back(dw);
+            R.rows.push_back(ok ? h.L[dw] : 0);
+            R.n_alns.push_back(ok ? (uint8_t)h.nsel[dw] : 0);
+            R.n_sup.push_back(ok ? h.nsup[dw] : 0);
+            R.n_ids.push_back(ok ? n1[dw] : 0);
+        }
+        // the reference batches: groups of -b windows in wid order, of which the windows with supported positions (k_ref_lmax)
+        for (uint32_t g0 = 0; g0 < nwin; g0 += bs) {
+            uint32_t B = 0, lmax = 0;
+            for (uint32_t k = g0; k < std::min(g0 + bs, nwin); k++)
+                if (R.n_sup[w_out0 + k]) { R.batch_win.push_back(w_out0 + k); B++; lmax = std::max(lmax, R.rows[w_out0 + k]); }
+            if (!B) continue;
+            R.batch_B.push_back(B);
+            R.batch_Lmax.push_back(lmax);
+            sh.n_batch_rows += (uint64_t)B * lmax;
+        }
+    }
+    for (size_t w = 0; w < R.rows.size(); w++) { sh.n_rows += R.rows[w]; sh.n_sup += R.n_sup[w]; sh.n_ids += R.n_ids[w]; }
+    if (R.rows.size() >= (1ull << 32) || sh.n_sup >= (1ull << 32)) return fail(ctx, HB_ERR_CAPACITY, "batch too large: 2^32 windows or positions");
+    sh.ticket = ++Fl.ticket;
+    sh.n_targets = n_targets;
+    sh.n_windows = (uint32_t)R.rows.size();
+    sh.n_batches = (uint32_t)R.batch_B.size();
+    sh.n_failed = n_failed;
+    R.shape = sh;
+    R.view = b;
+    R.valid = true;
+    *shape = sh;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    hb_stats& T = ctx->stats;
+    T.ms_features += ms_front;
+    T.kernel_launches += launches;
+    T.h2d_bytes += S.h2d_bytes;
+    T.d2h_bytes += S.d2h_bytes;
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    if (!first_err.empty()) ctx->err = first_err;
+    return HB_OK;
+}
+
+// The work of hb_features_fetch, with the lane's lock held and the context's device current
+int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream) {
+    hb_ctx::FeatLane& Fl = ctx->feat;
+    const FeatResult& R = Fl.res;
+    if (!shape || !out) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (out->struct_size != sizeof(hb_features_out)) return fail(ctx, HB_ERR_ARG, "hb_features_out.struct_size mismatch");
+    if (flags & ~HB_FEAT_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
+    if (!R.valid || shape->ticket != R.shape.ticket) return fail(ctx, HB_ERR_STATE, "the shape is not the context's latest hb_features_batch result");
+    const bool dev = (flags & HB_FEAT_DEVICE_PTRS) != 0;
+    {
+        const void* p[15] = {out->bases, out->quals, out->batch_bases, out->batch_quals, out->status, out->n_windows, out->rows, out->n_alns,
+                             out->n_sup, out->n_ids, out->supported, out->indices, out->ids, out->batch_B, out->batch_Lmax};
+        static const char* name[15] = {"bases", "quals", "batch_bases", "batch_quals", "status", "n_windows", "rows", "n_alns", "n_sup",
+                                       "n_ids", "supported", "indices", "ids", "batch_B", "batch_Lmax"};
+        for (int i = 0; i < 16; i++) {
+            const void* q = i < 15 ? p[i] : out->batch_win;
+            if (!q) continue;
+            const int k = pointer_kind(q, ctx->device);
+            const char* nm = i < 15 ? name[i] : "batch_win";
+            if (dev && i < 4 && k != 1)
+                return fail(ctx, HB_ERR_ARG, std::string(nm) + " is not memory of device " + std::to_string(ctx->device) + " (HB_FEAT_DEVICE_PTRS is set)");
+            if ((!dev || i >= 4) && k != 0)
+                return fail(ctx, HB_ERR_ARG, std::string(nm) + " is device memory" + (i < 4 ? " (HB_FEAT_DEVICE_PTRS is not set)" : ""));
+        }
+    }
+    const hb_features_shape& sh = R.shape;
+    const size_t nt = sh.n_targets, nw = sh.n_windows;
+    // ---- the metadata, from the host tables
+    if (out->status && nt) memcpy(out->status, R.status.data(), nt * 4);
+    if (out->n_windows && nt) memcpy(out->n_windows, R.n_windows.data(), nt * 4);
+    if (out->rows && nw) memcpy(out->rows, R.rows.data(), nw * 4);
+    if (out->n_alns && nw) memcpy(out->n_alns, R.n_alns.data(), nw);
+    if (out->n_sup && nw) memcpy(out->n_sup, R.n_sup.data(), nw * 4);
+    if (out->n_ids && nw) memcpy(out->n_ids, R.n_ids.data(), nw * 4);
+    if (out->batch_B && sh.n_batches) memcpy(out->batch_B, R.batch_B.data(), (size_t)sh.n_batches * 4);
+    if (out->batch_Lmax && sh.n_batches) memcpy(out->batch_Lmax, R.batch_Lmax.data(), (size_t)sh.n_batches * 4);
+    if (out->batch_win && !R.batch_win.empty()) memcpy(out->batch_win, R.batch_win.data(), R.batch_win.size() * 4);
+    const bool want_rows = (out->bases || out->quals) && sh.n_rows, want_batch = (out->batch_bases || out->batch_quals) && sh.n_batch_rows;
+    const bool want_lists = ((out->supported || out->indices) && sh.n_sup) || (out->ids && sh.n_ids);
+    if (!want_rows && !want_batch && !want_lists) return HB_OK;
+    // ---- the tables of the output kernels: the ragged rows, the batch slots, the lists
+    const BatchView& b = R.view;
+    size_t n_rseg = 0, n_bseg = 0, n_lseg = 0;
+    for (size_t w = 0; w < nw; w++) {
+        if (R.rows[w]) n_rseg++;
+        if (R.n_sup[w] || R.n_ids[w]) n_lseg++;
+    }
+    n_bseg = R.batch_win.size();
+    Carve ct{nullptr};
+    RowSeg *t_rows, *t_batch;
+    ListSeg* t_lists;
+    ct(t_rows, n_rseg); ct(t_batch, n_bseg); ct(t_lists, n_lseg);
+    const size_t tab_bytes = ct.bytes;
+    CK(Fl.pin_tab.grow(tab_bytes));
+    CK(Fl.d_tab.grow(tab_bytes));
+    Carve hc{Fl.pin_tab.as<uint8_t>()}, dc{Fl.d_tab.as<uint8_t>()};
+    RowSeg *h_rows, *h_batch, *d_rows, *d_batch;
+    ListSeg *h_lists, *d_lists;
+    hc(h_rows, n_rseg); hc(h_batch, n_bseg); hc(h_lists, n_lseg);
+    dc(d_rows, n_rseg); dc(d_batch, n_bseg); dc(d_lists, n_lseg);
+    {
+        uint64_t orow = 0, osup = 0, oid = 0;
+        size_t kr = 0, kl = 0;
+        for (size_t w = 0; w < nw; w++) {
+            const uint32_t dw = R.dev_win[w];
+            if (R.rows[w]) h_rows[kr++] = RowSeg{orow, R.dev_rowbase[dw], R.rows[w], R.rows[w]};
+            if (R.n_sup[w] || R.n_ids[w]) h_lists[kl++] = ListSeg{dw, 0, osup, oid};
+            orow += R.rows[w]; osup += R.n_sup[w]; oid += R.n_ids[w];
+        }
+        uint64_t brow = 0;
+        size_t ks = 0;
+        for (size_t k = 0; k < R.batch_B.size(); k++) {
+            for (uint32_t s = 0; s < R.batch_B[k]; s++, ks++) {
+                const uint32_t w = R.batch_win[ks];
+                h_batch[ks] = RowSeg{brow + (uint64_t)s * R.batch_Lmax[k], R.dev_rowbase[R.dev_win[w]], R.rows[w], R.batch_Lmax[k]};
+            }
+            brow += (uint64_t)R.batch_B[k] * R.batch_Lmax[k];
+        }
+    }
+    // ---- where the kernels write: the caller's device memory, or the staging region the host-bound outputs are copied from
+    uint8_t *o_b = nullptr, *o_q = nullptr, *o_bb = nullptr, *o_bq = nullptr;
+    uint32_t *o_sup = nullptr, *o_ids = nullptr;
+    int32_t* o_idx = nullptr;
+    {
+        const size_t rb = want_rows ? sh.n_rows * R_COLS : 0, bb = want_batch ? sh.n_batch_rows * R_COLS : 0;
+        Carve oc{nullptr};
+        uint8_t *s_b, *s_q, *s_bb, *s_bq;
+        uint32_t *s_sup, *s_ids;
+        int32_t* s_idx;
+        auto lay = [&](Carve& c) {
+            c(s_b, dev || !out->bases ? 0 : rb); c(s_q, dev || !out->quals ? 0 : rb);
+            c(s_bb, dev || !out->batch_bases ? 0 : bb); c(s_bq, dev || !out->batch_quals ? 0 : bb);
+            c(s_sup, out->supported ? sh.n_sup * 2 : 0); c(s_idx, out->indices ? sh.n_sup : 0); c(s_ids, out->ids ? sh.n_ids : 0);
+        };
+        lay(oc);
+        CK(Fl.d_out.grow(oc.bytes));
+        Carve c{Fl.d_out.as<uint8_t>()};
+        lay(c);
+        o_b = !out->bases || !want_rows ? nullptr : dev ? out->bases : s_b;
+        o_q = !out->quals || !want_rows ? nullptr : dev ? out->quals : s_q;
+        o_bb = !out->batch_bases || !want_batch ? nullptr : dev ? out->batch_bases : s_bb;
+        o_bq = !out->batch_quals || !want_batch ? nullptr : dev ? out->batch_quals : s_bq;
+        o_sup = out->supported && sh.n_sup ? s_sup : nullptr;
+        o_idx = out->indices && sh.n_sup ? s_idx : nullptr;
+        o_ids = out->ids && sh.n_ids ? s_ids : nullptr;
+    }
+    // ---- device work
+    hb_ctx::Lane* L = &Fl.lane;
+    KTimer& kt = L->kt;
+    kt.discard();
+    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
+    kt.st = L->stream;
+    if (dev) {
+        CK(cudaEventRecord(L->ev[3], (cudaStream_t)stream));
+        CK(cudaStreamWaitEvent(L->stream, L->ev[3], 0));
+    }
+    CK(cudaMemcpyAsync(Fl.d_tab.p, Fl.pin_tab.p, tab_bytes, cudaMemcpyHostToDevice, L->stream));
+    CK(cudaEventRecord(L->ev[4], L->stream));
+    uint64_t launches = 0;
+    if (o_b || o_q) { kt.begin(K_LISTS); launch_rows_out(d_rows, (uint32_t)n_rseg, b.mat_bases, b.mat_quals, o_b, o_q, L->stream); kt.end(); launches++; }
+    if (o_bb || o_bq) { kt.begin(K_LISTS); launch_rows_out(d_batch, (uint32_t)n_bseg, b.mat_bases, b.mat_quals, o_bb, o_bq, L->stream); kt.end(); launches++; }
+    if (o_sup || o_idx || o_ids) { kt.begin(K_LISTS); launch_lists_out(b, d_lists, (uint32_t)n_lseg, o_sup, o_idx, o_ids, L->stream); kt.end(); launches++; }
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(L->ev[5], L->stream));
+    // ---- host-bound outputs straight into the caller's memory
+    uint64_t d2h = 0;
+    auto copy = [&](void* dst, const void* src, size_t bytes) -> int {
+        if (!dst || !src || !bytes) return HB_OK;
+        CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, L->stream));
+        d2h += bytes;
+        return HB_OK;
+    };
+    int rc = HB_OK;
+    if (!dev) {
+        if (!rc) rc = copy(out->bases, o_b, sh.n_rows * R_COLS);
+        if (!rc) rc = copy(out->quals, o_q, sh.n_rows * R_COLS);
+        if (!rc) rc = copy(out->batch_bases, o_bb, sh.n_batch_rows * R_COLS);
+        if (!rc) rc = copy(out->batch_quals, o_bq, sh.n_batch_rows * R_COLS);
+    }
+    if (!rc) rc = copy(out->supported, o_sup, sh.n_sup * 8);
+    if (!rc) rc = copy(out->indices, o_idx, sh.n_sup * 4);
+    if (!rc) rc = copy(out->ids, o_ids, sh.n_ids * 4);
+    if (rc) { kt.discard(); return rc; }
+    CK(cudaStreamSynchronize(L->stream));
+    // ---- counters
+    hb_stats S{};
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, L->ev[4], L->ev[5]));
+    kt.collect(S.ms_kernel, S.n_kernel);
+    kt.on = false;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    hb_stats& T = ctx->stats;
+    T.ms_features += ms;
+    T.kernel_launches += launches;
+    T.h2d_bytes += tab_bytes;
+    T.d2h_bytes += d2h;
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    return HB_OK;
+}
+
 }  // namespace
 
 // ========================================================================================
@@ -1718,7 +2113,8 @@ int hb_inspect_model_ex(const char* model_path, uint32_t dims[9], uint64_t* para
 const char* hb_last_error(hb_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_err.c_str(); }
 
 int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_options* opt) {
-    if (!out || !model_path) { g_create_err = "null argument"; return HB_ERR_ARG; }
+    const bool no_model = opt && opt->struct_size == sizeof(hb_options) && (opt->flags & HB_FLAG_NO_MODEL);
+    if (!out || (!model_path && !no_model)) { g_create_err = "null argument"; return HB_ERR_ARG; }
     *out = nullptr;
     hb_ctx* ctx = new hb_ctx();
     ctx->device = cuda_device;
@@ -1776,6 +2172,15 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
             if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
         Cn.d_in.st = Cn.d_out.st = Cn.stream;
     }
+    {
+        auto& Fl = ctx->feat;
+        auto& L = Fl.lane;
+        if (cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
+        for (auto& e : L.ev)
+            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
+        L.d_batch.st = L.d_rows.st = L.d_fwd.st = Fl.d_tab.st = Fl.d_out.st = L.stream;
+        Fl.hbt = HostBatch(cuda_device);
+    }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
         cudaMemPool_t pool;
         uint64_t keep = UINT64_MAX;
@@ -1783,8 +2188,11 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
             cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
     }
     if (features_configure(ctx->opt.window_size) != cudaSuccess) { ctx->err = "kernel attribute setup failed (not an sm_90a device?)"; return bail(HB_ERR_CUDA); }
-    int rc = load_weights(ctx, model_path);
-    if (rc) return bail(rc);
+    ctx->no_model = no_model;
+    if (!no_model) {
+        const int rc = load_weights(ctx, model_path);
+        if (rc) return bail(rc);
+    }
     ctx->generation = g_ctx_generation.fetch_add(1);
     for (int i = 0; i < ctx->n_lanes; i++) ctx->lanes[i].worker = std::thread(worker_main, ctx, i);
     *out = ctx;
@@ -1803,12 +2211,14 @@ void hb_destroy(hb_ctx* ctx) {
     for (auto& L : ctx->lanes) if (L.stream) cudaStreamSynchronize(L.stream);
     if (ctx->fwd.stream) cudaStreamSynchronize(ctx->fwd.stream);
     if (ctx->cons.stream) cudaStreamSynchronize(ctx->cons.stream);
+    if (ctx->feat.lane.stream) cudaStreamSynchronize(ctx->feat.lane.stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
     DevBuf* bufs[] = {&ctx->d_words, &ctx->d_word_off, &ctx->d_len, &ctx->d_qual, &ctx->d_qual_off, &ctx->d_ln};
     for (DevBuf* b : bufs) b->release();
     for (auto& L : ctx->lanes) L.release();
     ctx->fwd.release();
     ctx->cons.release();
+    ctx->feat.release();
     ctx->pin_in.release();
     ctx->slots.clear();
     ctx->queue.clear();
@@ -1895,6 +2305,7 @@ int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_wo
 int hb_submit_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_overlap* ovl, uint32_t n_ovl,
                      const hb_overlap_window* ow, uint32_t n_ow) {
     if (!ctx) return HB_ERR_ARG;
+    if (ctx->no_model) return no_model_fail(ctx);
     thread_local PreparedTarget P;  // its vectors keep their capacity from target to target
     P.raw = false;
     t_err_sink = nullptr;
@@ -1910,51 +2321,13 @@ int hb_submit_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_ove
 
 int hb_submit_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_t n_ovl) {
     if (!ctx) return HB_ERR_ARG;
-    auto fail_locked = [&](int code, const std::string& msg) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = msg; return code; };
-    if (!ctx->have_reads) return fail_locked(HB_ERR_STATE, "hb_upload_reads must be called before submitting targets");
-    if (rid >= ctx->n_reads) return fail_locked(HB_ERR_ARG, "rid out of range");
-    if (n_ovl && !ovl) return fail_locked(HB_ERR_ARG, "null array");
-    const uint32_t W = ctx->opt.window_size;
-    const uint32_t n_windows = (ctx->read_len[rid] + W - 1) / W;
-    if (ctx->host_windowing) {  // A-B path: extract_windows on the calling thread, then the hb_submit_target route
-        std::vector<hb_overlap_window> ows;
-        for (uint32_t i = 0; i < n_ovl; i++) {
-            if (ovl[i].tid != rid) return fail_locked(HB_ERR_ARG, "overlap.tid != rid");
-            if (host_extract_windows(ovl[i], i, W, n_windows, ows) != 0)
-                return fail_locked(HB_ERR_INPUT, "malformed alignment (CIGAR / coordinates) for target " + std::to_string(rid));
-        }
-        return hb_submit_target(ctx, rid, n_windows, ovl, n_ovl, ows.data(), (uint32_t)ows.size());
-    }
-    // Device windowing (windowing_dev.cu): the host only lays out which (alignment, window) pairs exist — a function of the PAF
-    // coordinates — and ships the CIGARs; a CIGAR that is malformed or disagrees with its coordinates fails this target at
-    // hb_poll_corrected (HB_ERR_INPUT) instead of here.
+    if (ctx->no_model) return no_model_fail(ctx);
     thread_local PreparedTarget P;  // scratch reused across calls
-    thread_local std::vector<uint32_t> first, fill;
-    P.raw = true;
-    P.rid = rid; P.n_windows = n_windows; P.len = ctx->read_len[rid];
-    P.win_begin.assign(n_windows + 1, 0);
-    P.aln_now.assign(n_ovl, 0);
-    first.assign(n_ovl, 0);
-    uint64_t cb = 0;
-    for (uint32_t i = 0; i < n_ovl; i++) {
-        if (ovl[i].tid != rid) return fail_locked(HB_ERR_ARG, "overlap.tid != rid (alignments must be grouped by target)");
-        if (ovl[i].qid >= ctx->n_reads) return fail_locked(HB_ERR_ARG, "overlap.qid out of range");
-        if (!ovl[i].cigar && ovl[i].cigar_len) return fail_locked(HB_ERR_ARG, "null cigar");
-        if (ovl[i].strand > 1) return fail_locked(HB_ERR_ARG, "strand must be 0 or 1");
-        uint32_t wa, we;
-        if (skeleton_for_alignment(ovl[i], W, n_windows, wa, we) != 0)
-            return fail_locked(HB_ERR_INPUT, "malformed alignment (coordinates) for target " + std::to_string(rid));
-        first[i] = wa;
-        P.aln_now[i] = we - wa;
-        if (we > wa) cb += ovl[i].cigar_len;
-        for (uint32_t w = wa; w < we; w++) P.win_begin[w + 1]++;
-    }
-    for (uint32_t w = 0; w < n_windows; w++) P.win_begin[w + 1] += P.win_begin[w];
-    P.cig_bytes = cb;
-    P.ow.resize(P.win_begin[n_windows]);
-    fill.assign(P.win_begin.begin(), P.win_begin.end() - 1);
-    for (uint32_t i = 0; i < n_ovl; i++)  // alignment order inside every window = the reference's push order
-        for (uint32_t w = first[i]; w < first[i] + P.aln_now[i]; w++) P.ow[fill[w]++] = DevOW{i, w, 0, 0, 0, 0, 0, 0, 0, 0};
+    std::string local_err;  // validation errors are written to a local string first: ctx->err is shared between feature threads
+    t_err_sink = &local_err;
+    const int rc = prepare_alignments(ctx, rid, ovl, n_ovl, P);
+    t_err_sink = nullptr;
+    if (rc) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = local_err; return rc; }
     return stage_target(ctx, P, ovl, n_ovl);
 }
 
@@ -1989,6 +2362,7 @@ int hb_set_kernel_timing(hb_ctx* ctx, int on) {
 
 int hb_flush(hb_ctx* ctx) {
     if (!ctx) return HB_ERR_ARG;
+    if (ctx->no_model) return no_model_fail(ctx);
     std::unique_lock<std::mutex> lk(ctx->mu);
     {
         const uint32_t lt = ctx->opt.launch_targets, ns = std::max<uint32_t>(1u, (uint32_t)ctx->slots.size());
@@ -2396,6 +2770,7 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
 int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
                      const int32_t* indices, float* info_logits, float* bases_logits, uint32_t flags, void* stream) {
     if (!ctx) return HB_ERR_ARG;
+    if (ctx->no_model) return no_model_fail(ctx);
     std::lock_guard<std::mutex> lk(ctx->fwd.mu);
     int prev = -1;
     cudaGetDevice(&prev);
@@ -2425,6 +2800,43 @@ int hb_consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows,
     if (rc == HB_OK)
         rc = consensus_batch(ctx, n_reads, n_windows, rows, n_alns, bases, n_sup, supported, bases_logits, seqs, seg_len, n_segs, flags,
                              stream);
+    t_err_sink = nullptr;
+    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
+    if (rc != HB_OK) {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        ctx->err = err;
+    }
+    return rc;
+}
+
+int hb_features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const uint32_t* n_ovl, const hb_overlap* ovl,
+                      hb_features_shape* shape) {
+    if (!ctx) return HB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->feat.mu);
+    int prev = -1;
+    cudaGetDevice(&prev);
+    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
+    t_err_sink = &err;
+    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
+    if (rc == HB_OK) rc = features_batch(ctx, n_targets, rids, n_ovl, ovl, shape);
+    t_err_sink = nullptr;
+    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
+    if (rc != HB_OK) {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        ctx->err = err;
+    }
+    return rc;
+}
+
+int hb_features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream) {
+    if (!ctx) return HB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->feat.mu);
+    int prev = -1;
+    cudaGetDevice(&prev);
+    std::string err;
+    t_err_sink = &err;
+    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
+    if (rc == HB_OK) rc = features_fetch(ctx, shape, out, flags, stream);
     t_err_sink = nullptr;
     if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
     if (rc != HB_OK) {

@@ -194,6 +194,15 @@ struct ConsInArgs {
 };
 void launch_cons_in(const ConsInArgs& a, uint32_t n_win, cudaStream_t st);
 
+// feat_out.cu: the outputs of hb_features_batch.  A RowSeg is `total` output rows from out_row on: the first `valid` are the
+// arena's rows from src_row on, the rest padding (token 11 / quality 126).  A ListSeg puts window `win`'s supported list at entry
+// sup_out of (pos, ins) / indices and its surviving overlaps' query reads at entry id_out of ids.  Any output may be NULL.
+struct RowSeg { uint64_t out_row, src_row; uint32_t valid, total; };
+struct ListSeg { uint32_t win, pad; uint64_t sup_out, id_out; };
+void launch_rows_out(const RowSeg* seg, uint32_t n_seg, const uint8_t* mat_b, const uint8_t* mat_q, uint8_t* out_b, uint8_t* out_q,
+                     cudaStream_t st);
+void launch_lists_out(const BatchView& b, const ListSeg* seg, uint32_t n_seg, uint32_t* sup, int32_t* idx, uint32_t* ids, cudaStream_t st);
+
 // features.cu
 cudaError_t features_configure(uint32_t W);
 int launch_features_a(const BatchView& b, cudaStream_t st, KTimer& kt);

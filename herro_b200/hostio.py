@@ -196,6 +196,28 @@ class FeatureBatch:
     indices: list        # B arrays of i32 rows: target_rows[pos] + ins
 
 
+FEATURE_ASCII = np.frombuffer(b"ACGT*acgt#..", dtype=np.uint8)  # BASES_MAP inverted; token 11 (and anything above) as '.'
+SUPPORTED_DTYPE = np.dtype([("pos", "<u2"), ("ins", "u1")])    # SupportedPos (src/features.rs:894-898)
+
+
+def write_feature_window(read_dir: str, wid: int, tokens, quals, supported, id_names):
+    """The `herro features` files of one window (src/features.rs:724-764,806-839) under read_dir: <wid>.features.npy (u8 [2, L, 31]:
+    plane 0 the pileup as ASCII, plane 1 the qualities), <wid>.supported.npy (SupportedPos records) and <wid>.ids.txt (one read
+    name per surviving overlap, in final rank order), written with numpy's .npy writer.  tokens / quals [L, 31] u8, supported
+    [n, 2] (pos, ins), id_names: bytes."""
+    os.makedirs(read_dir, exist_ok=True)
+    tokens = np.asarray(tokens, dtype=np.uint8)
+    feats = np.stack([FEATURE_ASCII[np.minimum(tokens, 11)], np.asarray(quals, dtype=np.uint8)]).astype(np.uint8)
+    np.save(os.path.join(read_dir, f"{wid}.features.npy"), feats)
+    sup_in = np.asarray(supported).reshape(-1, 2)
+    sup = np.zeros(len(sup_in), dtype=SUPPORTED_DTYPE)
+    sup["pos"] = sup_in[:, 0]
+    sup["ins"] = sup_in[:, 1]
+    np.save(os.path.join(read_dir, f"{wid}.supported.npy"), sup)
+    with open(os.path.join(read_dir, f"{wid}.ids.txt"), "wb") as f:
+        f.write(b"".join(n + b"\n" for n in id_names))
+
+
 def read_feature_window(read_dir: str, wid: int):
     """-> (tokens [L, 31] u8, quals [L, 31] u8, indices [n] i32) of one window of a `herro features` read directory."""
     feats = np.load(os.path.join(read_dir, f"{wid}.features.npy"))

@@ -10,7 +10,7 @@
  *   inference::inference_worker     src/inference.rs:177-212  (spawned at src/lib.rs:189-196)
  *   consensus::consensus_worker     src/consensus.rs:229-263  (spawned at src/lib.rs:198-199)
  *
- * (all three at once through hb_submit_*; the model call and consensus also one at a time: hb_forward_batch, hb_consensus_batch)
+ * (all three at once through hb_submit_*; each also alone: hb_features_batch, hb_forward_batch, hb_consensus_batch)
  * with calls into this library (INTEGRATION.md shows the Rust side).  Plain pointers and
  * sizes only; no torch types; never unwinds or aborts (the reference is `panic = "abort"`,
  * Cargo.toml:14-16): every entry point returns HB_OK or a negative hb_status, and
@@ -78,6 +78,8 @@ typedef struct hb_options {
 } hb_options;
 
 #define HB_FLAG_KEEP_DEBUG 1u /* keep per-window intermediates of the last launch for hb_debug_*        */
+#define HB_FLAG_NO_MODEL   2u /* load no weights (model_path may be NULL): hb_features_batch and hb_consensus_batch only;   */
+                              /* hb_submit_*, hb_flush and hb_forward_batch return HB_ERR_STATE                          */
 
 typedef struct hb_ctx hb_ctx; /* one per GPU: streams, weights, read-store replica, staging buffers */
 
@@ -85,7 +87,9 @@ typedef struct hb_ctx hb_ctx; /* one per GPU: streams, weights, read-store repli
  * src/inference.rs:185).  `model_path` is what `-m` names: a TorchScript archive (`torch.jit.save`; ZIP with stored
  * entries + data.pkl, read natively, no libtorch) of a module with the architecture this library implements
  * (oracle/forward_ref.py naming; an optional `stem_bn` is folded), or the HB200W1 blob of herro_b200/weights.py.
- * Any other graph is HB_ERR_MODEL with the first missing parameter named: TorchScript code is not executed. */
+ * Any other graph is HB_ERR_MODEL with the first missing parameter named: TorchScript code is not executed.
+ * With HB_FLAG_NO_MODEL in opt->flags no weights are loaded and model_path may be NULL (it is ignored): such a context runs
+ * the features stage and consensus around a model the host executes itself (hb_features_batch, hb_consensus_batch). */
 int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_options* opt);
 void hb_destroy(hb_ctx* ctx);
 
@@ -121,6 +125,81 @@ int hb_submit_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_ove
  * coordinates) is reported for its target by hb_poll_corrected (HB_ERR_INPUT), not by this call; coordinate errors
  * (inverted ranges, windows past the end of the target) still fail here. */
 int hb_submit_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_t n_ovl);
+
+/* ---- the features stage alone ------------------------------------------------------------ */
+#define HB_FEAT_DEVICE_PTRS 1u /* hb_features_fetch: bases, quals, batch_bases and batch_quals are device pointers on the context's device */
+
+typedef struct hb_features_shape {  /* what one hb_features_batch produced                                                   */
+    uint64_t ticket;                /* names the result for hb_features_fetch                                                */
+    uint32_t n_targets, n_windows, n_batches, n_failed;
+    uint64_t n_rows, n_sup, n_ids;  /* N = sum rows, S = sum n_sup, sum n_ids                                                */
+    uint64_t n_batch_rows;          /* sum over the reference batches of B * Lmax                                            */
+} hb_features_shape;
+
+typedef struct hb_features_out {    /* = sizeof(hb_features_out); any other pointer may be NULL: that output is not written  */
+    uint32_t struct_size;
+    int32_t*  status;      /* [n_targets] host: HB_OK, HB_ERR_INPUT or HB_ERR_CAPACITY                                       */
+    uint32_t* n_windows;   /* [n_targets] host: ceil(len / W), n_total_wins                                                  */
+    uint32_t* rows;        /* [n_windows] host: L' of each window; 0 for the windows of a failed target                      */
+    uint8_t*  n_alns;      /* [n_windows] host: min(n_ids, 30)                                                               */
+    uint32_t* n_sup;       /* [n_windows] host: supported positions                                                          */
+    uint32_t* n_ids;       /* [n_windows] host: overlaps that survived the filter                                            */
+    uint8_t*  bases;       /* [N][31] BASES_MAP tokens, window after window      (host; device with HB_FEAT_DEVICE_PTRS)     */
+    uint8_t*  quals;       /* [N][31] raw quality bytes                          (host; device with HB_FEAT_DEVICE_PTRS)     */
+    uint32_t* supported;   /* [S][2] host: (pos, ins), window after window                                                   */
+    int32_t*  indices;     /* [S] host: the row of each supported entry inside its window (collate's indices)                */
+    uint32_t* ids;         /* [sum n_ids] host: query read id of every surviving overlap, in final rank order, window after window */
+    uint32_t* batch_B;     /* [n_batches] host: windows in each reference batch                                              */
+    uint32_t* batch_Lmax;  /* [n_batches] host: its longest window                                                           */
+    uint32_t* batch_win;   /* [sum batch_B] host: the window (index into the window order above) of each batch slot          */
+    uint8_t*  batch_bases; /* [n_batch_rows][31] tokens, padded with 11          (host; device with HB_FEAT_DEVICE_PTRS)     */
+    uint8_t*  batch_quals; /* [n_batch_rows][31] quality bytes, padded with 126  (host; device with HB_FEAT_DEVICE_PTRS)     */
+} hb_features_out;
+
+/* The replacement of extract_features (src/features.rs:326-583) on many targets at once, for a host that keeps its own model call
+ * (and perhaps its own consensus): what the reference's feature threads compute, without the model call and consensus that
+ * hb_submit_* chain onto it.  The input is hb_submit_alignments' for n_targets targets: target i is rids[i] with the n_ovl[i]
+ * alignments that follow those of target i-1 in `ovl` (every tid == rid), windowed on the device as hb_submit_alignments does.
+ * hb_features_batch computes and fills *shape with the sizes of every output; hb_features_fetch then copies out any subset of
+ * them, as often as wanted (for example the metadata first, then the bulk arrays into buffers of the sizes it gave).
+ *
+ * The windows: every target has all of its ceil(len / W) windows, in wid order, also those without alignments; targets in the
+ * order given.  Per window, exactly the arguments of FeaturesOutput::update (src/features.rs:570-578): the [L', 31] tokens and
+ * qualities, the (pos, ins) SupportedPos list with the row each entry names (collate's indices), and the ids.
+ * The reference batches: each target's windows are taken `-b` (hb_options.batch_size) at a time in wid order, as
+ * FeaturesOutput::update hands them to InferenceOutput::update; the windows of a group with at least one supported position form one
+ * batch (prepare_examples), padded to its longest window with token 11 and quality 126 (collate, src/inference.rs:73-140,214-250).
+ * batch_bases / batch_quals are those [B, Lmax, 31] tensors back to back, batch_win says which window each slot holds, and the
+ * indices of slot k are those of window batch_win[k]: the arguments of hb_forward_batch, whose output in turn orders the logits the
+ * way hb_consensus_batch takes them.
+ *
+ * Per-target failures (the call still returns HB_OK; hb_last_error names the first failed target): a malformed CIGAR or coordinates
+ * the reference would panic on are HB_ERR_INPUT, more than 60000 overlap-windows covering one window HB_ERR_CAPACITY.  A failed
+ * target keeps its n_windows, and its windows have no rows, positions or ids; it has no batches.  The other targets are unaffected.
+ *
+ * Errors of the call (the previous result is gone; nothing is written; the context stays usable):
+ *   HB_ERR_ARG       a NULL pointer, a rid out of range, an alignment with tid != rid, a qid out of range or a strand other than 0 / 1;
+ *                    for fetch also a struct_size mismatch, unknown flags, or a pointer that does not match the flag (bulk outputs
+ *                    must be device memory of the context's device with HB_FEAT_DEVICE_PTRS and host memory without; the others
+ *                    host memory always)
+ *   HB_ERR_STATE     no hb_upload_reads yet; for fetch, a shape whose ticket is not the context's latest result
+ *   HB_ERR_CAPACITY  a batch too large (2^32 CIGAR op slots, as a launch), or scratch that could not grow
+ *   HB_ERR_CUDA      a CUDA failure
+ *
+ * Synchronous: both calls return when their work is done.  With HB_FEAT_DEVICE_PTRS the library's stream first waits, through an
+ * event, for the work already enqueued on `stream` (NULL: the legacy default stream), so a caller can hand over freshly allocated
+ * tensors.  Scratch only grows, so repeated calls of the same or a smaller shape allocate nothing.  Host-bound bulk outputs are copied
+ * straight into the caller's memory.  A result stays valid until the next hb_features_batch on the context.
+ *
+ * Threading: calls of hb_features_batch / hb_features_fetch on one context serialise among themselves on a lane of their own; they may
+ * run beside hb_submit_*, hb_flush, hb_poll_corrected, hb_forward_batch and hb_consensus_batch (not beside hb_upload_reads), and never
+ * touch the pipeline's scratch, the debug taps or the launch hb_replay_last_launch re-runs.
+ *
+ * Counters: adds to kernel_launches, n_kernel / ms_kernel (the output kernels under HB_K_LISTS), ms_features, h2d_bytes, d2h_bytes
+ * and host_allocs when scratch grows; targets, windows, rows, supported and corrected_bases are untouched. */
+int hb_features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const uint32_t* n_ovl, const hb_overlap* ovl,
+                      hb_features_shape* shape);
+int hb_features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream);
 
 /* ---- the model call alone ---------------------------------------------------------------- */
 #define HB_FWD_DEVICE_PTRS 1u  /* bases, quals and both outputs are device pointers on the context's device */
