@@ -95,6 +95,9 @@ def load_library():
     L.hb_destroy.argtypes = [vp]
     L.hb_destroy.restype = None
     L.hb_upload_reads.argtypes = [vp, u32, vp, vp, vp]
+    L.hb_read_store_create.argtypes = [C.POINTER(vp), u32, vp, vp, vp]
+    L.hb_read_store_destroy.argtypes = [vp]
+    L.hb_attach_read_store.argtypes = [vp, vp]
     L.hb_submit_target.argtypes = [vp, u32, u32, vp, u32, vp, u32]
     L.hb_submit_alignments.argtypes = [vp, u32, vp, u32]
     L.hb_extract_windows.argtypes = [vp, u32, u32, u32, vp, u32, u32p]
@@ -129,7 +132,7 @@ EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
                     "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch",
-                    "hb_features_batch", "hb_features_fetch"]
+                    "hb_features_batch", "hb_features_fetch", "hb_read_store_create", "hb_read_store_destroy", "hb_attach_read_store"]
 HB_FWD_DEVICE_PTRS = 1
 HB_CONS_DEVICE_PTRS = 1
 HB_FEAT_DEVICE_PTRS = 1
@@ -302,6 +305,77 @@ class Features:
         return (self.n_windows, self.rows, self.n_alns, self.bases, _split(self.supported, self.n_sup), bases_logits)
 
 
+@dataclass
+class _Packed:
+    n: int
+    lens: np.ndarray   # u32 [n]
+    words: np.ndarray  # u64, all reads
+    woff: np.ndarray   # u64 [n+1]
+    quals: np.ndarray  # u8, all reads
+    wp: np.ndarray     # u64 [n]: address of each read's words
+    qp: np.ndarray     # u64 [n]: address of each read's qualities
+
+
+def _pack_reads(seqs, quals, off) -> _Packed:
+    """Concatenated ASCII / Phred+33 bytes with off[n+1] -> the HAECSeq layout (as get_reads packs it, src/haec_io.rs:56) and the
+    per-read pointer arrays hb_upload_reads and hb_read_store_create take."""
+    n = len(off) - 1
+    lens = np.diff(off).astype(np.uint32)
+    woff = np.zeros(n + 1, dtype=np.uint64)
+    woff[1:] = np.cumsum((lens.astype(np.uint64) + 31) // 32)
+    words = np.zeros(int(woff[-1]) + 1, dtype=np.uint64)
+    seqs = np.ascontiguousarray(seqs, dtype=np.uint8)
+    off64 = np.ascontiguousarray(off, dtype=np.uint64)
+    if _host_lib().hbh_pack_2bit(seqs.ctypes.data, off64.ctypes.data, n, words.ctypes.data, woff.ctypes.data,
+                                 min(os.cpu_count() or 1, 32)) != 0:
+        raise ValueError("non-ACGT base: the reference's 2-bit packing is undefined for it (SURVEY.md H12)")
+    quals = np.ascontiguousarray(quals, dtype=np.uint8)
+    wp = (words.ctypes.data + woff[:-1] * 8).astype(np.uint64)
+    qp = (quals.ctypes.data + off64[:-1]).astype(np.uint64)
+    return _Packed(n, lens, words, woff, quals, wp, qp)
+
+
+class ReadStore:
+    """The reads in pinned, device-mapped host memory (hb_read_store_create), for read sets larger than a GPU's memory: attach it to
+    any number of contexts on any devices (Context.attach_read_store) instead of uploading a copy to each.  Arguments as
+    Context.upload_reads.  close() frees it; it fails (HerroError, HB_ERR_STATE) while a context is still attached."""
+
+    def __init__(self, seqs: np.ndarray, quals: np.ndarray, off: np.ndarray):
+        p = _pack_reads(seqs, quals, off)
+        self._init(p.n, p.wp.ctypes.data, p.lens, p.qp.ctypes.data)
+
+    @classmethod
+    def _create(cls, n, word_ptrs, lens_ptr, qual_ptrs):
+        """From the per-read pointer arrays of a packed store (hostio.Reads.host_store)."""
+        self = cls.__new__(cls)
+        lens = np.ctypeslib.as_array(C.cast(lens_ptr, C.POINTER(C.c_uint32)), (n,)).copy() if n else np.zeros(0, np.uint32)
+        self._init(n, word_ptrs, lens, qual_ptrs, lens_ptr)
+        return self
+
+    def _init(self, n, word_ptrs, lens, qual_ptrs, lens_ptr=None):
+        self._L = load_library()
+        self._h = C.c_void_p()
+        self.n = n
+        self.lens = lens
+        rc = self._L.hb_read_store_create(C.byref(self._h), n, word_ptrs, lens_ptr if lens_ptr is not None else lens.ctypes.data,
+                                          qual_ptrs)
+        if rc != 0:
+            raise HerroError(rc, self._L.hb_last_error(None).decode())
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            rc = self._L.hb_read_store_destroy(self._h)
+            if rc != 0:
+                raise HerroError(rc, self._L.hb_last_error(None).decode())
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Context:
     """One per GPU — the per-device worker group of src/lib.rs:154-200."""
 
@@ -322,11 +396,13 @@ class Context:
         self._keep = []
         self.read_len = None
         self.failed = []
+        self._store = None
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
             self._L.hb_destroy(self._h)
             self._h = C.c_void_p()
+        self._store = None
 
     def __del__(self):
         try:
@@ -343,22 +419,20 @@ class Context:
     def upload_reads(self, seqs: np.ndarray, quals: np.ndarray, off: np.ndarray):
         """seqs/quals: concatenated ASCII / Phred+33 bytes, off[n+1].  Packs to the HAECSeq
         layout on the host (as get_reads does, src/haec_io.rs:56) and replicates it on the GPU."""
-        n = len(off) - 1
-        lens = np.diff(off).astype(np.uint32)
-        woff = np.zeros(n + 1, dtype=np.uint64)
-        woff[1:] = np.cumsum((lens.astype(np.uint64) + 31) // 32)
-        words = np.zeros(int(woff[-1]) + 1, dtype=np.uint64)
-        seqs = np.ascontiguousarray(seqs, dtype=np.uint8)
-        off64 = np.ascontiguousarray(off, dtype=np.uint64)
-        if _host_lib().hbh_pack_2bit(seqs.ctypes.data, off64.ctypes.data, n, words.ctypes.data, woff.ctypes.data,
-                                     min(os.cpu_count() or 1, 32)) != 0:
-            raise ValueError("non-ACGT base: the reference's 2-bit packing is undefined for it (SURVEY.md H12)")
-        quals = np.ascontiguousarray(quals, dtype=np.uint8)
-        wp = (words.ctypes.data + woff[:-1] * 8).astype(np.uint64)
-        qp = (quals.ctypes.data + off[:-1].astype(np.uint64)).astype(np.uint64)
-        self._check(self._L.hb_upload_reads(self._h, n, wp.ctypes.data, lens.ctypes.data, qp.ctypes.data))
-        self.read_len = lens
-        self.packed_words, self.packed_word_off = words, woff
+        p = _pack_reads(seqs, quals, off)
+        self._check(self._L.hb_upload_reads(self._h, p.n, p.wp.ctypes.data, p.lens.ctypes.data, p.qp.ctypes.data))
+        self.read_len = p.lens
+        self.packed_words, self.packed_word_off = p.words, p.woff
+        self._store = None
+
+    def attach_read_store(self, store: "ReadStore"):
+        """Use a read store in pinned host memory instead of an uploaded copy (hb_attach_read_store): each launch gathers only its
+        own reads over PCIe.  The context keeps a reference to the store, so the store outlives it."""
+        if not isinstance(store, ReadStore) or not store._h.value:
+            raise TypeError("store must be an open ReadStore")
+        self._check(self._L.hb_attach_read_store(self._h, store._h))
+        self._store = store
+        self.read_len = store.lens
 
     # -- submission ---------------------------------------------------------------------
     @staticmethod

@@ -10,7 +10,9 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
                                        (consensus alone, on `features` and `predict` output)
 
 Nothing is computed here: FASTQ parsing / 2-bit packing, `*.oec.zst` decoding and PAF parsing, the feature / consumer threads
-and the FASTA writer are C++ threads (hbh_inference); `features` and `inference --torch` call hb_features_batch.  In deployment this
+and the FASTA writer are C++ threads (hbh_inference); `features` and `inference --torch` call hb_features_batch.  Each command keeps
+the reads in pinned host memory instead of device memory when they take more than half of the smallest selected GPU's memory
+(hostio.host_store_above).  In deployment this
 role is played by the unchanged Rust binary (INTEGRATION.md); the flags keep the reference's meaning: reads shorter than `-w`
 are not loaded (src/haec_io.rs:48), unknown names / self overlaps / repeated (query,target) pairs are skipped
 (src/overlaps.rs:137-185), `-c` cluster files restrict targets to core reads (:154-159).
@@ -65,7 +67,7 @@ def features(args):
     R = hostio.Reads(args.reads, min_len=args.window_size)
     A = hostio.Alignments(args.read_alns, R)
     ctx = api.Context(None, 0, args.window_size, 64)
-    R.upload(ctx)
+    R.load_into(ctx, hostio.device_bytes([0]))
     n = 0
     step = max(1, args.targets_per_launch)
     for k0 in range(0, A.n_targets, step):
@@ -98,7 +100,7 @@ def inference_torch(args):
     R = hostio.Reads(args.reads, min_len=args.window_size)
     A = hostio.Alignments(args.read_alns, R)
     ctx = api.Context(None, dev, args.window_size, args.batch_size)
-    R.upload(ctx)
+    R.load_into(ctx, hostio.device_bytes([dev]))
     cuda = torch.device("cuda", dev)
     module = torch.jit.load(args.model, map_location=cuda).eval()
     out = hostio.FastaWriter(args.output)

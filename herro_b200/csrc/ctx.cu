@@ -175,6 +175,11 @@ struct FwdBufs {  // the forward region's arrays besides the work list, which is
     uint8_t* ws;
 };
 
+struct GatherSizes {  // host store: the arrays k_reads_in fills in a launch's batch region; n_reads == 0: the uploaded store
+    uint32_t n_reads = 0, n_list = 0;
+    uint64_t words = 0, qual = 0;
+};
+
 struct LastLaunch {  // host copies of per-window metadata of the most recent launch (debug taps / replay)
     bool valid = false;
     std::vector<DevWin> win;
@@ -186,8 +191,10 @@ struct LastLaunch {  // host copies of per-window metadata of the most recent la
     // the counts the lane's scratch was carved from, besides those in `view` (a pre-sized lane carves the view again)
     size_t cig_bytes = 0;
     uint64_t op_slots = 0, raw_slots = 0;
+    GatherSizes gs;
     BatchView view;
     FwdBufs fwd;
+    ReadsInArgs gather{};  // host store: the gather the launch began with (replays run it again)
 };
 
 // What one hb_features_batch produced, in the caller's order (targets as given, each target's windows in wid order).  The bulk
@@ -206,6 +213,18 @@ struct FeatResult {
 
 }  // namespace
 
+// The read store in host memory (hb_read_store_create): every read's words and qualities in one page-locked block that every
+// device of the process can map, each read 16-byte aligned and padded to 16 bytes (zero words, quality 33), so that k_reads_in
+// moves whole 16-byte vectors.
+struct hb_read_store {
+    uint8_t* block = nullptr;                  // cudaHostAlloc(Portable | Mapped): the words of all reads, then their qualities
+    uint64_t words_bytes = 0, bytes = 0;
+    std::vector<uint64_t> word_off, qual_off;  // per read, in words / bytes from the start of each section
+    std::vector<uint32_t> len;
+    uint32_t n_reads = 0, max_len = 0;
+    std::atomic<uint32_t> attached{0};         // contexts using the store; it must outlive them
+};
+
 struct hb_ctx {
     int device = 0;
     hb_options opt{};
@@ -222,7 +241,10 @@ struct hb_ctx {
     std::vector<uint32_t> read_len;
     DevBuf d_words, d_word_off, d_len, d_qual, d_qual_off, d_ln;
     uint32_t ln_n = 0;
-    ReadStoreView rs{};
+    ReadStoreView rs{};  // with a host store only len and n: each launch views its gathered reads
+    hb_read_store* store = nullptr;  // hb_attach_read_store; nullptr: the uploaded store above
+    const uint64_t* store_words = nullptr;  // the store's sections as this device maps them
+    const uint8_t* store_qual = nullptr;
 
     // staging: every submitting (feature) thread fills its own batch without taking the context lock;
     // full batches are handed to the launch worker's queue
@@ -243,9 +265,14 @@ struct hb_ctx {
         uint64_t seen_sizes = 0;  // version of hb_ctx::lane_sizes this lane has been pre-sized to
         LastLaunch last;
         std::thread worker;
+        // host store: the read list of the launch being staged, and a stamp per read that marks it listed
+        PinVec<ReadCopy> read_list;
+        std::vector<uint32_t> stamp;
+        uint32_t stamp_gen = 0;
         void release() {
             d_batch.release(); d_rows.release(); d_fwd.release();
             pin_small.release(); pin_out.release();
+            read_list.release();
             for (auto& e : ev) if (e) cudaEventDestroy(e);
             kt.destroy();
             if (stream) cudaStreamDestroy(stream);
@@ -639,8 +666,10 @@ struct Carve {
 };
 
 // Batch region, sized from the HostBatch when a launch starts (the view's n_tgt / n_win / n_ovl / n_ow and W, and the CIGAR
-// bytes and op slots): inputs, raw and tokenised ops, everything per overlap-window, overlap, window and target, counters.
-size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t raw_slots, uint8_t* base) {
+// bytes and op slots): inputs, raw and tokenised ops, everything per overlap-window, overlap, window and target, counters.  With a
+// host store also the launch's gathered reads, their read list and the offset tables, which become the view's read store.
+size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t raw_slots, const GatherSizes& gs, ReadsInArgs& g,
+                   uint8_t* base) {
     const size_t nt = b.n_tgt, nw = b.n_win, no1 = std::max<size_t>(b.n_ovl, 1), ow1 = std::max<size_t>(b.n_ow, 1);
     const size_t ops = std::max<uint64_t>(op_slots, 1), raw = std::max<uint64_t>(raw_slots, 1);
     Carve c{base};
@@ -685,6 +714,20 @@ size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t r
     c(b.w_outoff, nw);
     c(b.tgt_err, nt);
     c(b.counters, CNT_N);
+    if (gs.n_reads) {
+        c(g.list, gs.n_list);
+        c(g.words, READS_FRONT_WORDS + gs.words + READS_BACK_WORDS);
+        c(g.qual, READS_FRONT_QUAL + gs.qual + READS_BACK_QUAL);
+        c(g.word_off, (size_t)gs.n_reads + 1);
+        c(g.qual_off, (size_t)gs.n_reads + 1);
+        g.n = gs.n_list;
+        g.n_words = gs.words;
+        g.n_qual = gs.qual;
+        b.rs.words = g.words + READS_FRONT_WORDS;
+        b.rs.word_off = g.word_off;
+        b.rs.qual = g.qual + READS_FRONT_QUAL;
+        b.rs.qual_off = g.qual_off;
+    }
     return c.bytes;
 }
 
@@ -731,7 +774,8 @@ size_t carve_readback(Readback& h, size_t nt, size_t nw, uint8_t* base) {
     return c.bytes;
 }
 
-// The counts of a launch and the context's read store; the scratch pointers are carved from the lane's regions.
+// The counts of a launch and the context's read store (with a host store, carve_batch points it at the gathered reads); the scratch
+// pointers are carved from the lane's regions.
 BatchView make_view(hb_ctx* ctx, const HostBatch& hbt) {
     BatchView b{};
     b.rs = ctx->rs;
@@ -836,20 +880,55 @@ uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw
 #define SYNC_TIMED() do { const double t__ = now_ms(); CK(cudaStreamSynchronize(L->stream)); t_wait += now_ms() - t__; } while (0)
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
 
+// Host store: the distinct reads of a staged batch (its targets and every query), each listed once in L->read_list with its place
+// in the store and in the batch region, reads laid out in order of first appearance.
+int list_reads(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, GatherSizes& gs) {
+    const hb_read_store* st = ctx->store;
+    if (L->stamp.size() != st->n_reads) { L->stamp.assign(st->n_reads, 0); L->stamp_gen = 0; }
+    if (++L->stamp_gen == 0) { std::fill(L->stamp.begin(), L->stamp.end(), 0u); L->stamp_gen = 1; }
+    const uint32_t gen = L->stamp_gen;
+    PinVec<ReadCopy>& list = L->read_list;
+    list.clear();
+    if (!list.reserve(std::min<size_t>(hbt.tgt.size() + hbt.ovl.size(), st->n_reads)))
+        return fail(ctx, HB_ERR_CAPACITY, "out of pinned host memory (read list)");
+    uint64_t dw = 0, dq = 0;
+    auto add = [&](uint32_t r) {
+        if (L->stamp[r] == gen) return;
+        L->stamp[r] = gen;
+        const uint32_t len = st->len[r];
+        list.p[list.n++] = ReadCopy{st->word_off[r], st->qual_off[r], dw, dq, r, len};
+        dw += ((uint64_t)len + 63) / 64 * 2;
+        dq += ((uint64_t)len + 15) / 16 * 16;
+    };
+    for (const DevTarget& t : hbt.tgt) add(t.rid);
+    for (const DevOverlap& o : hbt.ovl) add(o.qid);
+    gs = GatherSizes{st->n_reads, (uint32_t)list.size(), dw, dq};
+    return HB_OK;
+}
+
 // The front half of a launch, shared by run_batch and hb_features_batch: carve the batch region for the staged batch, copy it in,
-// and run windowing, the pileup and the per-window lists until the row arena holds every row (it is regrown on overflow).  On
-// return `b` views the lane's regions, h.cnt / h.nsup hold the counts of the last attempt, ev[0] / ev[2] bracket its feature
-// kernels, and *total_rows is the rows of all windows.
+// gather its reads from a host store, and run windowing, the pileup and the per-window lists until the row arena holds every row
+// (it is regrown on overflow).  On return `b` views the lane's regions, h.cnt / h.nsup hold the counts of the last attempt,
+// ev[0] / ev[2] bracket its feature kernels (the gather included), *total_rows is the rows of all windows, and gs / g describe the
+// gather (gs.n_reads == 0 without a host store).
 int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, Readback& h, uint64_t* launches, uint64_t* total_rows,
-              hb_stats& S, double& t_wait, double& t_mark) {
+              GatherSizes& gs, ReadsInArgs& g, hb_stats& S, double& t_wait, double& t_mark) {
     const uint32_t W = ctx->opt.window_size;
     const size_t nt = hbt.tgt.size(), nw = hbt.win.size();
     const size_t cig_bytes = hbt.cig.size();
     const uint64_t op_slots = hbt.op_cap + hbt.dev_op_cap, raw_slots = hbt.raw_cap;
     if (op_slots >= 0xffffffffull) return fail(ctx, HB_ERR_CAPACITY, "batch too large: more than 2^32 CIGAR ops (lower launch_targets)");
+    gs = GatherSizes{};
+    g = ReadsInArgs{};
+    if (ctx->store) {
+        const int rc = list_reads(ctx, L, hbt, gs);
+        if (rc) return rc;
+        g.src_words = ctx->store_words;
+        g.src_qual = ctx->store_qual;
+    }
     b = make_view(ctx, hbt);
-    CK(L->d_batch.grow(carve_batch(b, cig_bytes, op_slots, raw_slots, nullptr)));
-    carve_batch(b, cig_bytes, op_slots, raw_slots, L->d_batch.as<uint8_t>());
+    CK(L->d_batch.grow(carve_batch(b, cig_bytes, op_slots, raw_slots, gs, g, nullptr)));
+    carve_batch(b, cig_bytes, op_slots, raw_slots, gs, g, L->d_batch.as<uint8_t>());
     // ---- H2D straight from the pinned staging arrays of the batch
     const size_t sz[5] = {vbytes(hbt.tgt), vbytes(hbt.win), vbytes(hbt.ovl), vbytes(hbt.ow), hbt.cig.size()};
     const void* src[5] = {hbt.tgt.data(), hbt.win.data(), hbt.ovl.data(), hbt.ow.data(), hbt.cig.data()};
@@ -872,6 +951,11 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
         rc = zero_scratch(ctx, L, b);
         if (rc) return rc;
         CK(cudaEventRecord(L->ev[0], L->stream));
+        if (gs.n_reads && attempt == 0) {  // a regrown row arena leaves the batch region, and the gathered reads, as they are
+            CK(cudaMemcpyAsync((void*)g.list, L->read_list.data(), vbytes(L->read_list), cudaMemcpyHostToDevice, L->stream));
+            *launches += launch_reads_in(g, L->stream, L->kt);
+            S.h2d_bytes += vbytes(L->read_list) + gs.words * 8 + gs.qual;
+        }
         *launches += launch_features_a(b, L->stream, L->kt);
         CK(cudaEventRecord(L->ev[1], L->stream));
         *launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
@@ -907,7 +991,9 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     Readback h;
     uint64_t launches = 0;
     uint64_t total_rows = 0;
-    int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, S, t_wait, t_mark);
+    GatherSizes gs;
+    ReadsInArgs g;
+    int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, gs, g, S, t_wait, t_mark);
     if (rc) return rc;
     const uint64_t n_sup = (uint64_t)h.cnt[CNT_NSUP] | ((uint64_t)h.cnt[CNT_NSUP + 1] << 32);
     const uint32_t max_nsup = nw ? *std::max_element(h.nsup, h.nsup + nw) : 0;
@@ -1013,8 +1099,10 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     ll.cig_bytes = cig_bytes;
     ll.op_slots = op_slots;
     ll.raw_slots = raw_slots;
+    ll.gs = gs;
     ll.view = b;
     ll.fwd = f;
+    ll.gather = g;
     S.ms_worker_busy = now_ms() - t_begin;
     S.ms_worker_gpu_wait = t_wait;
     {
@@ -1146,7 +1234,7 @@ void presize_lane(hb_ctx* ctx, hb_ctx::Lane* L, const hb_ctx::LaneSizes& T) {
     cudaStreamSynchronize(L->stream);
     LastLaunch& ll = L->last;
     if (ll.valid) {  // the regions moved with their contents: carving the kept view's counts again gives the same offsets
-        carve_batch(ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, L->d_batch.as<uint8_t>());
+        carve_batch(ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, ll.gs, ll.gather, L->d_batch.as<uint8_t>());
         carve_rows(ll.view, L->d_rows.as<uint8_t>());
         const uint32_t max_nsup = ll.w_nsup.empty() ? 0 : *std::max_element(ll.w_nsup.begin(), ll.w_nsup.end());
         carve_fwd(ctx, ll.view, ll.fwd, ll.n_sup, max_nsup, L->d_fwd.as<uint8_t>());
@@ -1832,7 +1920,9 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
     double t_wait = 0, t_mark = now_ms();
     float ms_front = 0;
     if (nt) {
-        int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, S, t_wait, t_mark);
+        GatherSizes gs;
+        ReadsInArgs g;
+        int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, gs, g, S, t_wait, t_mark);
         if (rc) { L->kt.discard(); return rc; }
         CK(Fl.pin_n1.grow(nw * 4));
         uint32_t* n1 = Fl.pin_n1.as<uint32_t>();
@@ -1842,7 +1932,6 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
         CK(cudaMemcpyAsync(n1, b.w_n1, nw * 4, cudaMemcpyDeviceToHost, L->stream));
         CK(cudaStreamSynchronize(L->stream));
         CK(cudaEventElapsedTime(&ms_front, L->ev[0], L->ev[2]));
-        S.h2d_bytes = vbytes(hbt.tgt) + vbytes(hbt.win) + vbytes(hbt.ovl) + vbytes(hbt.ow) + hbt.cig.size();
         S.d2h_bytes = CNT_N * 4 + nw * 16 + nt * 4;
         L->kt.collect(S.ms_kernel, S.n_kernel);
         L->kt.on = false;
@@ -2074,6 +2163,30 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     return HB_OK;
 }
 
+// ---------------------------------------------------------------------------------- read store
+// ln(k) table from the host libm — the value Rust's f64::ln returns (src/features.rs:507)
+int upload_ln_table(hb_ctx* ctx, uint32_t max_len) {
+    ctx->ln_n = max_len + 2;
+    std::vector<double> ln(ctx->ln_n);
+    ln[0] = 0.0;
+    for (uint32_t k = 1; k < ctx->ln_n; k++) ln[k] = std::log((double)k);
+    CK(ctx->d_ln.grow((size_t)ctx->ln_n * 8));
+    CK(cudaMemcpy(ctx->d_ln.p, ln.data(), (size_t)ctx->ln_n * 8, cudaMemcpyHostToDevice));
+    return HB_OK;
+}
+
+// Leave the host store (lock held, context idle).  The lanes' last launches would gather from it again when replayed: they are
+// dropped, and the context has no reads until the caller's upload or attach completes.
+void detach_store(hb_ctx* ctx) {
+    ctx->store->attached.fetch_sub(1);
+    ctx->store = nullptr;
+    ctx->store_words = nullptr;
+    ctx->store_qual = nullptr;
+    ctx->have_reads = false;
+    for (auto& L : ctx->lanes) L.last.valid = false;
+    ctx->last_lane = -1;
+}
+
 }  // namespace
 
 // ========================================================================================
@@ -2213,6 +2326,7 @@ void hb_destroy(hb_ctx* ctx) {
     if (ctx->cons.stream) cudaStreamSynchronize(ctx->cons.stream);
     if (ctx->feat.lane.stream) cudaStreamSynchronize(ctx->feat.lane.stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
+    if (ctx->store) ctx->store->attached.fetch_sub(1);
     DevBuf* bufs[] = {&ctx->d_words, &ctx->d_word_off, &ctx->d_len, &ctx->d_qual, &ctx->d_qual_off, &ctx->d_ln};
     for (DevBuf* b : bufs) b->release();
     for (auto& L : ctx->lanes) L.release();
@@ -2235,6 +2349,7 @@ int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_wo
         if (!sl->batch.tgt.empty()) return fail(ctx, HB_ERR_STATE, "hb_upload_reads with targets pending: call hb_flush first");
     if (!seq_words || !seq_len || !qual || n_reads == 0) return fail(ctx, HB_ERR_ARG, "null/empty read store");
     CK(cudaSetDevice(ctx->device));
+    if (ctx->store) detach_store(ctx);
     std::vector<uint64_t> woff(n_reads + 1, 0), qoff(n_reads + 1, 0);
     uint32_t max_len = 0;
     for (uint32_t i = 0; i < n_reads; i++) {
@@ -2286,18 +2401,104 @@ int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_wo
     CK(cudaMemcpy(ctx->d_word_off.p, woff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->d_qual_off.p, qoff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->d_len.p, seq_len, (size_t)n_reads * 4, cudaMemcpyHostToDevice));
-    // ln(k) table from the host libm — the value Rust's f64::ln returns (src/features.rs:507)
-    ctx->ln_n = max_len + 2;
-    std::vector<double> ln(ctx->ln_n);
-    ln[0] = 0.0;
-    for (uint32_t k = 1; k < ctx->ln_n; k++) ln[k] = std::log((double)k);
-    CK(ctx->d_ln.grow((size_t)ctx->ln_n * 8));
-    CK(cudaMemcpy(ctx->d_ln.p, ln.data(), (size_t)ctx->ln_n * 8, cudaMemcpyHostToDevice));
+    rc = upload_ln_table(ctx, max_len);
+    if (rc) return rc;
     ctx->stats.h2d_bytes += woff[n_reads] * 8 + qoff[n_reads];
     ctx->n_reads = n_reads;
     ctx->read_len.assign(seq_len, seq_len + n_reads);
     ctx->rs = ReadStoreView{ctx->d_words.as<uint64_t>() + FRONT_WORDS, ctx->d_word_off.as<uint64_t>(), ctx->d_len.as<uint32_t>(),
                             ctx->d_qual.as<uint8_t>() + FRONT_QUAL, ctx->d_qual_off.as<uint64_t>(), n_reads};
+    ctx->have_reads = true;
+    return HB_OK;
+}
+
+int hb_read_store_create(hb_read_store** out, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
+                         const uint8_t* const* qual) {
+    g_create_err.clear();
+    if (!out || !seq_words || !seq_len || !qual || n_reads == 0) { g_create_err = "null/empty read store"; return HB_ERR_ARG; }
+    *out = nullptr;
+    for (uint32_t i = 0; i < n_reads; i++)
+        if (!seq_words[i] || !qual[i]) { g_create_err = "null read"; return HB_ERR_ARG; }
+    std::unique_ptr<hb_read_store> s(new hb_read_store());
+    s->n_reads = n_reads;
+    s->len.assign(seq_len, seq_len + n_reads);
+    s->word_off.resize(n_reads);
+    s->qual_off.resize(n_reads);
+    uint64_t w = 0, q = 0;
+    for (uint32_t i = 0; i < n_reads; i++) {
+        s->word_off[i] = w;
+        s->qual_off[i] = q;
+        w += ((uint64_t)seq_len[i] + 63) / 64 * 2;
+        q += ((uint64_t)seq_len[i] + 15) / 16 * 16;
+        s->max_len = std::max(s->max_len, seq_len[i]);
+    }
+    s->words_bytes = w * 8;
+    s->bytes = s->words_bytes + q;
+    const cudaError_t e = cudaHostAlloc((void**)&s->block, std::max<uint64_t>(s->bytes, 16), cudaHostAllocPortable | cudaHostAllocMapped);
+    if (e != cudaSuccess) {
+        s->block = nullptr;
+        g_create_err = std::string("cudaHostAlloc of the read store (") + std::to_string(s->bytes) + " bytes): " + cudaGetErrorString(e);
+        return e == cudaErrorMemoryAllocation ? HB_ERR_CAPACITY : HB_ERR_CUDA;
+    }
+    // every read with its padding: zero words up to an even count, quality 33 up to a multiple of 16 (the uploaded store's pad values)
+    uint64_t* words = (uint64_t*)s->block;
+    uint8_t* quals = s->block + s->words_bytes;
+    const hb_read_store& S = *s;
+    auto copy = [&](uint32_t i0, uint32_t i1) {
+        for (uint32_t i = i0; i < i1; i++) {
+            const uint64_t nw = ((uint64_t)seq_len[i] + 31) / 32, sw = ((uint64_t)seq_len[i] + 63) / 64 * 2;
+            memcpy(words + S.word_off[i], seq_words[i], nw * 8);
+            memset(words + S.word_off[i] + nw, 0, (sw - nw) * 8);
+            const uint64_t sq = ((uint64_t)seq_len[i] + 15) / 16 * 16;
+            memcpy(quals + S.qual_off[i], qual[i], seq_len[i]);
+            memset(quals + S.qual_off[i] + seq_len[i], 33, sq - seq_len[i]);
+        }
+    };
+    const uint32_t nth = std::min<uint32_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<uint32_t>(16u, n_reads));
+    std::vector<std::thread> th;
+    for (uint32_t t = 0; t < nth; t++) th.emplace_back(copy, (uint32_t)((uint64_t)n_reads * t / nth), (uint32_t)((uint64_t)n_reads * (t + 1) / nth));
+    for (auto& t : th) t.join();
+    *out = s.release();
+    return HB_OK;
+}
+
+int hb_read_store_destroy(hb_read_store* store) {
+    if (!store) { g_create_err = "null read store"; return HB_ERR_ARG; }
+    if (store->attached.load()) { g_create_err = "the read store is still attached to a context"; return HB_ERR_STATE; }
+    cudaFreeHost(store->block);
+    delete store;
+    return HB_OK;
+}
+
+int hb_attach_read_store(hb_ctx* ctx, hb_read_store* store) {
+    if (!ctx) return HB_ERR_ARG;
+    std::unique_lock<std::mutex> lk(ctx->mu);
+    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
+    for (auto& sl : ctx->slots)
+        if (!sl->batch.tgt.empty()) return fail(ctx, HB_ERR_STATE, "hb_attach_read_store with targets pending: call hb_flush first");
+    if (!store) return fail(ctx, HB_ERR_ARG, "null read store");
+    CK(cudaSetDevice(ctx->device));
+    void* dp = nullptr;
+    CK(cudaHostGetDevicePointer(&dp, store->block, 0));
+    if (ctx->store) detach_store(ctx);
+    // the uploaded store's HBM is what this mode gives back
+    for (DevBuf* b : {&ctx->d_words, &ctx->d_word_off, &ctx->d_qual, &ctx->d_qual_off}) b->release();
+    for (auto& L : ctx->lanes) L.last.valid = false;  // their views point into the freed store
+    ctx->last_lane = -1;
+    ctx->have_reads = false;
+    const uint32_t n = store->n_reads;
+    CK(ctx->d_len.grow((size_t)n * 4));
+    CK(cudaMemcpy(ctx->d_len.p, store->len.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+    const int rc = upload_ln_table(ctx, store->max_len);
+    if (rc) return rc;
+    ctx->stats.h2d_bytes += (uint64_t)n * 4 + (uint64_t)ctx->ln_n * 8;
+    store->attached.fetch_add(1);
+    ctx->store = store;
+    ctx->store_words = (const uint64_t*)dp;
+    ctx->store_qual = (const uint8_t*)dp + store->words_bytes;
+    ctx->n_reads = n;
+    ctx->read_len = store->len;
+    ctx->rs = ReadStoreView{nullptr, nullptr, ctx->d_len.as<uint32_t>(), nullptr, nullptr, n};
     ctx->have_reads = true;
     return HB_OK;
 }
@@ -2753,6 +2954,7 @@ int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
     for (uint32_t it = 0; it < iters; it++) {
         int rc = zero_scratch(ctx, L, b);
         if (rc) return rc;
+        if (L->last.gs.n_reads) launches += launch_reads_in(L->last.gather, L->stream, L->kt);
         launches += launch_features_a(b, L->stream, L->kt);
         launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
         launches += launch_features_c1(b, L->stream, L->kt);

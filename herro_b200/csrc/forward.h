@@ -203,6 +203,24 @@ void launch_rows_out(const RowSeg* seg, uint32_t n_seg, const uint8_t* mat_b, co
                      cudaStream_t st);
 void launch_lists_out(const BatchView& b, const ListSeg* seg, uint32_t n_seg, uint32_t* sup, int32_t* idx, uint32_t* ids, cudaStream_t st);
 
+// reads_in.cu: a launch's reads from the host read store (device-mapped host memory) into its batch region.  The region's arrays
+// keep the uploaded store's padding: `words` is READS_FRONT_WORDS zero words, n_words gathered words, READS_BACK_WORDS zero words;
+// `qual` likewise in bytes of 33.  Every offset is in words / bytes from the first gathered one, and 16-byte aligned: in the store
+// and in the region each read takes its words and qualities rounded up to 16 bytes.
+constexpr uint32_t READS_FRONT_WORDS = 32, READS_BACK_WORDS = 8, READS_FRONT_QUAL = 256, READS_BACK_QUAL = 16;
+struct ReadCopy { uint64_t src_w, src_q, dst_w, dst_q; uint32_t rid, len; };
+struct ReadsInArgs {
+    const ReadCopy* list;
+    uint32_t n;
+    const uint64_t* src_words;        // the store's words and qualities (device-mapped pointers)
+    const uint8_t* src_qual;
+    uint64_t* words;                  // the region's padded arrays
+    uint8_t* qual;
+    uint64_t n_words, n_qual;
+    uint64_t *word_off, *qual_off;    // [n_reads + 1], written for the listed reads only
+};
+uint64_t launch_reads_in(const ReadsInArgs& a, cudaStream_t st, KTimer& kt);
+
 // features.cu
 cudaError_t features_configure(uint32_t W);
 int launch_features_a(const BatchView& b, cudaStream_t st, KTimer& kt);

@@ -11,7 +11,7 @@
 //                  library but no header) and parsed by its own worker.
 //   hbh_fasta_*    correction_writer / write_sequence (src/lib.rs:267-317): `>id[:k] description\n seq\n`
 //   hbh_inference  the whole `herro inference --read-alns` pipeline over the public C ABI of libherro_b200: ingest ->
-//                  hb_upload_reads -> feature threads (hb_submit_alignments) -> consumer (hb_poll_corrected) -> FASTA,
+//                  hb_upload_reads (or one host read store for all devices) -> feature threads (hb_submit_alignments) -> consumer (hb_poll_corrected) -> FASTA,
 //                  with the time of every stage reported.
 //
 // In the deployed layout these stay in the Rust host; they exist here because no Rust toolchain is available offline and
@@ -540,32 +540,63 @@ int hbh_fasta_close(hbh_fasta* w, uint64_t* records, uint64_t* bases) {
 }
 
 // ================================================================================================ the whole pipeline
+// Bytes of the packed read store (2-bit words and one quality byte per base), which `host_store_above` is compared with
+uint64_t hbh_reads_store_bytes(const hbh_reads* r) { return r->woff.back() * 8 + r->qoff.back(); }
+
 // `herro inference --read-alns <alns_dir> -m <model> -b <batch> -t <threads> -d <devices> [-c cluster] <reads> <output>` over the C ABI.
 // devices: n_dev CUDA device ids (targets are dealt to the devices' feature threads from one shared counter, like the
 // reference's per-device worker groups pulling one channel, src/lib.rs:154-187).
-// times8: FASTQ load, pack, alignment ingest (wall), read-store upload (max over devices), correction (first submit -> last
-// result), FASTA close, total wall, corrected bases.
+// host_store_above: when the packed store is larger than this many bytes, the reads stay in host memory (one hb_read_store that every
+// device attaches; the harness's own packed copy is freed once it exists), else every device gets an uploaded copy.
+// times8: FASTQ load, pack, alignment ingest (wall), read-store upload or host-store creation + attach (max over devices),
+// correction (first submit -> last result), FASTA close, total wall, corrected bases.
 int hbh_inference(const char* reads_path, const char* alns_dir, const char* model, const char* output, uint32_t window, uint32_t batch,
                   int threads, const int* devices, int n_dev, const char* const* core, uint32_t n_core, const char* const* neighbour,
-                  uint32_t n_neigh, int io_threads, double* times8, uint64_t* counts4) {
+                  uint32_t n_neigh, int io_threads, uint64_t host_store_above, double* times8, uint64_t* counts4) {
     if (!reads_path || !alns_dir || !model || !output || !devices || n_dev < 1) return HB_ERR_ARG;
     const double t_begin = now_s();
     hbh_reads* R = nullptr;
     int rc = hbh_reads_load(reads_path, window, core, n_core, neighbour, n_neigh, io_threads, &R);
     if (rc) return rc;
     // Context creation (CUDA initialisation, weights) and the read-store upload of every device run while the alignment batches are
-    // decompressed and parsed on the host: the two need nothing from each other (both only read `R`).
+    // decompressed and parsed on the host: the two need nothing from each other (both only read `R`; the alignments need only
+    // the names and lengths, so the packed words and qualities may go once a host store holds them).
     std::vector<hb_ctx*> ctx((size_t)n_dev, nullptr);
     hb_options opt{};
     opt.struct_size = sizeof opt; opt.window_size = window; opt.batch_size = batch;
     std::vector<double> t_up((size_t)n_dev, 0);
     hbh_alns* A = nullptr;
-    auto cleanup = [&]() { for (hb_ctx* c : ctx) if (c) hb_destroy(c); if (A) hbh_alns_free(A); hbh_reads_free(R); };
+    hb_read_store* store = nullptr;
+    auto cleanup = [&]() {
+        for (hb_ctx* c : ctx) if (c) hb_destroy(c);
+        if (store) hb_read_store_destroy(store);
+        if (A) hbh_alns_free(A);
+        hbh_reads_free(R);
+    };
     std::atomic<int> bad{0};
+    const bool host_store = hbh_reads_store_bytes(R) > host_store_above;
+    double t_store = 0;
+    std::string store_err;
+    std::thread store_th;
+    if (host_store)
+        store_th = std::thread([&]() {
+            const double t0 = now_s();
+            if (hb_read_store_create(&store, hbh_reads_count(R), hbh_reads_word_ptrs(R), hbh_reads_lens(R), hbh_reads_qual_ptrs(R)) != HB_OK) {
+                store_err = hb_last_error(nullptr);
+                bad = HB_ERR_CUDA;
+                return;
+            }
+            std::vector<uint64_t>().swap(R->words);
+            std::vector<uint8_t>().swap(R->qual);
+            R->word_ptr.assign(R->word_ptr.size(), nullptr);
+            R->qual_ptr.assign(R->qual_ptr.size(), nullptr);
+            t_store = now_s() - t0;
+        });
     std::vector<std::thread> dev_th;
     for (int d = 0; d < n_dev; d++)
         dev_th.emplace_back([&, d]() {
             if (hb_create(&ctx[d], devices[d], model, &opt) != HB_OK) { bad = HB_ERR_CUDA; return; }
+            if (host_store) return;
             const double t0 = now_s();
             if (hb_upload_reads(ctx[d], hbh_reads_count(R), hbh_reads_word_ptrs(R), hbh_reads_lens(R), hbh_reads_qual_ptrs(R)) != HB_OK) bad = HB_ERR_CUDA;
             t_up[d] = now_s() - t0;
@@ -575,9 +606,18 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
     const double t_ingest = now_s() - t_al0;
     const std::string ingest_err = rc ? t_err : std::string();
     for (auto& t : dev_th) t.join();
+    if (host_store) {
+        store_th.join();
+        for (int d = 0; d < n_dev && !bad.load(); d++) {
+            const double t0 = now_s();
+            if (hb_attach_read_store(ctx[d], store) != HB_OK) bad = HB_ERR_CUDA;
+            t_up[d] = t_store + now_s() - t0;
+        }
+    }
     if (rc) { t_err = ingest_err; cleanup(); return rc; }
     if (bad.load()) {
         t_err = "context creation / read-store upload failed";
+        if (!store_err.empty()) t_err += ": " + store_err;
         for (hb_ctx* c : ctx) if (c) { t_err += std::string(": ") + hb_last_error(c); break; }
         if (const char* ce = hb_last_error(nullptr)) if (*ce) t_err += std::string(": ") + ce;
         cleanup();

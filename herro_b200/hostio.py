@@ -44,7 +44,9 @@ def _lib():
     H.hbh_fasta_write.argtypes = [vp, C.c_char_p, C.c_char_p, vp, vp, u32]
     H.hbh_fasta_close.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     H.hbh_inference.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, u32, u32, C.c_int, vp, C.c_int, vp, u32, vp, u32,
-                                C.c_int, vp, vp]
+                                C.c_int, C.c_uint64, vp, vp]
+    H.hbh_reads_store_bytes.argtypes = [vp]
+    H.hbh_reads_store_bytes.restype = C.c_uint64
     H._io_ready = True
     return H
 
@@ -95,6 +97,26 @@ class Reads:
         ctx._check(ctx._L.hb_upload_reads(ctx._h, self.n, H.hbh_reads_word_ptrs(self._h), H.hbh_reads_lens(self._h),
                                           H.hbh_reads_qual_ptrs(self._h)))
         ctx.read_len = self.lens.copy()
+
+    def store_bytes(self) -> int:
+        """Bytes of the packed store: 2-bit words and one quality byte per base."""
+        return int(self._H.hbh_reads_store_bytes(self._h))
+
+    def host_store(self) -> "api.ReadStore":
+        """A read store in pinned host memory (hb_read_store_create) straight from the packed store (no copy through Python)."""
+        H = self._H
+        return api.ReadStore._create(self.n, H.hbh_reads_word_ptrs(self._h), H.hbh_reads_lens(self._h), H.hbh_reads_qual_ptrs(self._h))
+
+    def load_into(self, ctx: "api.Context", device_bytes, read_store=None):
+        """The reads into a context as `inference` chooses (host_store_above): uploaded, or attached as a host store, which is
+        returned (it must outlive the context)."""
+        if self.store_bytes() > host_store_above(device_bytes, read_store):
+            store = self.host_store()
+            ctx.attach_read_store(store)
+            ctx.read_len = self.lens.copy()
+            return store
+        self.upload(ctx)
+        return None
 
     def close(self):
         if self._h:
@@ -311,16 +333,38 @@ def feature_reads(features_dir: str):
             if os.path.isdir(os.path.join(features_dir, d)) and any(f.endswith(".features.npy") for f in os.listdir(os.path.join(features_dir, d)))]
 
 
+def host_store_above(device_bytes, read_store=None) -> int:
+    """The packed read-store size (bytes) above which the reads stay in pinned host memory (one hb_read_store for all devices)
+    instead of a copy in every device's memory: half the memory of the smallest selected device, which leaves the other half to
+    the model and the launches.  read_store "host" / "device" forces one of the two."""
+    if read_store == "host":
+        return 0
+    if read_store == "device":
+        return 2 ** 64 - 1
+    if read_store is not None:
+        raise ValueError(f"read_store must be None, 'host' or 'device', got {read_store!r}")
+    return min(int(b) for b in device_bytes) // 2
+
+
+def device_bytes(devices) -> list:
+    """Total memory of each CUDA device in `devices`."""
+    import torch
+    return [torch.cuda.get_device_properties(int(d)).total_memory for d in devices]
+
+
 def inference(reads_path: str, alns_dir: str, model: str, output: str, window: int = 4096, batch: int = 64, threads: int = 1,
-              devices=(0,), core=None, neighbour=None, io_threads: int = 0) -> dict:
-    """The reference's `herro inference --read-alns` command, natively (hbh_inference) -> stage times and counts."""
+              devices=(0,), core=None, neighbour=None, io_threads: int = 0, read_store=None) -> dict:
+    """The reference's `herro inference --read-alns` command, natively (hbh_inference) -> stage times and counts.  The read store
+    is chosen by host_store_above; read_store ("host" / "device") overrides it."""
     H = _lib()
     dev = np.asarray(list(devices), dtype=np.int32)
     ca, nc, k1 = _strs(core)
     na, nn, k2 = _strs(neighbour)
+    above = host_store_above(None if read_store else device_bytes(dev), read_store)
     t8, c4 = np.zeros(8), np.zeros(4, np.uint64)
     rc = H.hbh_inference(reads_path.encode(), alns_dir.encode(), model.encode(), output.encode(), window, batch, threads,
-                         dev.ctypes.data, len(dev), ca, nc, na, nn, io_threads or min(os.cpu_count() or 1, 32), t8.ctypes.data, c4.ctypes.data)
+                         dev.ctypes.data, len(dev), ca, nc, na, nn, io_threads or min(os.cpu_count() or 1, 32), above, t8.ctypes.data,
+                         c4.ctypes.data)
     if rc != 0:
         raise api.HerroError(rc, H.hbh_last_error().decode())
     return dict(fastq_load_s=t8[0], pack_s=t8[1], alignment_ingest_s=t8[2], read_store_upload_s=t8[3], correction_s=t8[4],

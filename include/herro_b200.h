@@ -108,6 +108,40 @@ int hb_inspect_model_ex(const char* model_path, uint32_t dims[9], uint64_t* para
 int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
                     const uint8_t* const* qual);
 
+/* ---- the read store in host memory ------------------------------------------------------ */
+/* For read sets larger than the GPU's memory (a 50x human set is ~200 GB packed): the reads stay in host RAM, as the reference keeps
+ * them (src/lib.rs:241-265), and every launch copies only its own reads to the device.
+ *
+ * hb_read_store_create takes hb_upload_reads' arguments and layout rules and copies the reads into ONE page-locked, portable,
+ * device-mapped host allocation (each read's words and qualities 16-byte aligned) that contexts on any GPU of the process share.
+ * It needs no context and does no GPU work; errors (HB_ERR_ARG for a NULL pointer, zero reads or a NULL read, checked before any
+ * CUDA call; HB_ERR_CAPACITY / HB_ERR_CUDA when the allocation fails) are reported through hb_last_error(NULL).  The caller's arrays
+ * may be freed once it returns: peak host memory is briefly twice the store.
+ *
+ * hb_attach_read_store replaces hb_upload_reads for one context: it frees a store uploaded earlier and uploads only len[]
+ * (4 * n_reads bytes) and the ln table (8 * (max_len + 2) bytes), which is all it adds to h2d_bytes.  Same preconditions as
+ * hb_upload_reads (HB_ERR_STATE with targets pending; not beside hb_features_batch).  A later hb_upload_reads or
+ * hb_attach_read_store detaches again; the launch hb_replay_last_launch would re-run is dropped by either.
+ *
+ * Lifetime: the store counts the contexts attached to it.  hb_read_store_destroy returns HB_ERR_STATE while any is (the store is
+ * then left intact and usable); hb_destroy detaches.  The store must outlive every context attached to it.
+ * Threading: any number of contexts, on any devices, may share one store and run at the same time; the store is read-only.
+ *
+ * What a launch (hb_submit_*, hb_features_batch) reads over PCIe: its distinct reads (targets and every query of its alignments),
+ * each read's words and qualities rounded up to 16 bytes, plus a read list of 40 bytes per read.  A kernel (k_reads_in) gathers
+ * them from the mapped store into the launch's scratch, so HBM use is set by the launch size (hb_set_launch_targets bounds it),
+ * not by the read set.  Scratch that cannot grow fails the launch's targets with HB_ERR_CAPACITY, as other scratch does.
+ * hb_replay_last_launch re-runs the gather too, so its time includes PCIe reads in this mode.
+ *
+ * Counters: h2d_bytes grows by the gathered bytes and the read list; the gather kernel counts under HB_K_LISTS and inside
+ * ms_features; building the read list is part of ms_worker_phase[0].
+ * Results: every output is identical to that of an uploaded store holding the same reads. */
+typedef struct hb_read_store hb_read_store;
+int hb_read_store_create(hb_read_store** out, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
+                         const uint8_t* const* qual);
+int hb_read_store_destroy(hb_read_store* store);
+int hb_attach_read_store(hb_ctx* ctx, hb_read_store* store);
+
 /* Submit one target read: the replacement of extract_features(rid, reads, overlaps, ...)
  * (src/features.rs:326-333) for a host that still runs windowing::extract_windows itself.
  * n_windows = ceil(len/W) (src/features.rs:338).  `ow` lists the OverlapWindows in the order
