@@ -10,7 +10,9 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
                                        (consensus alone, on `features` and `predict` output)
 
 Nothing is computed here: FASTQ parsing / 2-bit packing, `*.oec.zst` decoding and PAF parsing, the feature / consumer threads
-and the FASTA writer are C++ threads (hbh_inference); `features` and `inference --torch` call hb_features_batch.  Each command keeps
+and the FASTA writer are C++ threads (hbh_inference); `features` and `inference --torch` call hb_features_batch.  The alignment
+files are streamed: background workers decode and parse the next files, within 1/8 of physical memory (one larger file is still
+read whole), while the earlier ones are corrected, and each file is freed once its targets are submitted.  Each command keeps
 the reads in pinned host memory instead of device memory when they take more than half of the smallest selected GPU's memory
 (hostio.host_store_above).  In deployment this
 role is played by the unchanged Rust binary (INTEGRATION.md); the flags keep the reference's meaning: reads shorter than `-w`
@@ -65,19 +67,22 @@ def features(args):
     """`herro features` (src/lib.rs:50-111): the per-window feature files of every target, from hb_features_batch on a context
     without weights, `--targets-per-launch` targets per call."""
     R = hostio.Reads(args.reads, min_len=args.window_size)
-    A = hostio.Alignments(args.read_alns, R)
+    S = hostio.Alignments.stream(args.read_alns, R)
     ctx = api.Context(None, 0, args.window_size, 64)
     R.load_into(ctx, hostio.device_bytes([0]))
     n = 0
     step = max(1, args.targets_per_launch)
-    for k0 in range(0, A.n_targets, step):
-        F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))])
-        for k in range(len(F.rids)):
-            if F.status[k]:  # the reference would have panicked on this read's alignments
-                print(f"skipped read {os.fsdecode(R.ids[F.rids[k]])}: error {int(F.status[k])}", file=sys.stderr)
-                continue
-            write_features(F, k, args.output, R.ids)
-            n += 1
+    for A in S:
+        for k0 in range(0, A.n_targets, step):
+            F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))])
+            for k in range(len(F.rids)):
+                if F.status[k]:  # the reference would have panicked on this read's alignments
+                    print(f"skipped read {os.fsdecode(R.ids[F.rids[k]])}: error {int(F.status[k])}", file=sys.stderr)
+                    continue
+                write_features(F, k, args.output, R.ids)
+                n += 1
+        A.close()
+    S.close()
     ctx.close()
     print(f"Wrote the feature files of {n} reads under {args.output}.", file=sys.stderr)
 
@@ -98,33 +103,37 @@ def inference_torch(args):
     if "," in str(args.devices):
         raise SystemExit("--torch runs on one device (-d)")
     R = hostio.Reads(args.reads, min_len=args.window_size)
-    A = hostio.Alignments(args.read_alns, R)
+    S = hostio.Alignments.stream(args.read_alns, R)
     ctx = api.Context(None, dev, args.window_size, args.batch_size)
     R.load_into(ctx, hostio.device_bytes([dev]))
     cuda = torch.device("cuda", dev)
     module = torch.jit.load(args.model, map_location=cuda).eval()
     out = hostio.FastaWriter(args.output)
     step = max(1, args.targets_per_launch)
-    failed = 0
+    failed = targets = 0
     with torch.no_grad(), torch.cuda.device(cuda):
-        for k0 in range(0, A.n_targets, step):
-            F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))], device=True, batches=True)
-            logits = []
-            for _, bases, quals, lens, indices in F.batches():
-                idx = [torch.from_numpy(np.ascontiguousarray(i)).to(cuda) for i in indices]
-                _, bl = module(bases.to(torch.int32), quals_normalised(quals), torch.from_numpy(lens).to(cuda), idx)
-                logits.append(bl.float())
-            for k, segs in enumerate(ctx.consensus_batch(*F.consensus_args(logits))):
-                rid = F.rids[k]
-                if F.status[k]:
-                    failed += 1
-                elif segs:
-                    out.write(R.ids[rid], R.descriptions[rid], segs)
+        for A in S:
+            for k0 in range(0, A.n_targets, step):
+                F = ctx.features_batch([A.target(k) for k in range(k0, min(k0 + step, A.n_targets))], device=True, batches=True)
+                logits = []
+                for _, bases, quals, lens, indices in F.batches():
+                    idx = [torch.from_numpy(np.ascontiguousarray(i)).to(cuda) for i in indices]
+                    _, bl = module(bases.to(torch.int32), quals_normalised(quals), torch.from_numpy(lens).to(cuda), idx)
+                    logits.append(bl.float())
+                for k, segs in enumerate(ctx.consensus_batch(*F.consensus_args(logits))):
+                    rid = F.rids[k]
+                    if F.status[k]:
+                        failed += 1
+                    elif segs:
+                        out.write(R.ids[rid], R.descriptions[rid], segs)
+            targets += A.n_targets
+            A.close()
+    S.close()
     records, bases = out.close()
     ctx.close()
-    print(f"Processed {A.n_targets} reads, wrote {records} records ({bases} bases)" + (f"; skipped {failed} reads" if failed else ""),
+    print(f"Processed {targets} reads, wrote {records} records ({bases} bases)" + (f"; skipped {failed} reads" if failed else ""),
           file=sys.stderr)
-    return dict(targets=A.n_targets, records=records, corrected_bases=bases, failed_targets=failed)
+    return dict(targets=targets, records=records, corrected_bases=bases, failed_targets=failed)
 
 
 def predict(args):

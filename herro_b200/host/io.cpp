@@ -7,12 +7,13 @@
 //                  (overlaps::read_batches + parse_paf, src/overlaps.rs:288-323,117-202): header lines skipped, unknown read
 //                  names skipped, core filter on the target, self overlaps dropped, only the first line of an ordered
 //                  (query, target) pair per batch file kept.  The reference decodes and parses batch files one after the
-//                  other on one thread; here every file is decompressed (libzstd through dlopen: the image ships the
-//                  library but no header) and parsed by its own worker.
+//                  other on one thread; here workers decompress (libzstd through dlopen: the image ships the library but no
+//                  header) and parse upcoming files while earlier ones are used (hbh_alns_stream_*), within a budget of host
+//                  memory; hbh_alns_load is the same stream with no budget, merged.
 //   hbh_fasta_*    correction_writer / write_sequence (src/lib.rs:267-317): `>id[:k] description\n seq\n`
-//   hbh_inference  the whole `herro inference --read-alns` pipeline over the public C ABI of libherro_b200: ingest ->
-//                  hb_upload_reads (or one host read store for all devices) -> feature threads (hb_submit_alignments) -> consumer (hb_poll_corrected) -> FASTA,
-//                  with the time of every stage reported.
+//   hbh_inference  the whole `herro inference --read-alns` pipeline over the public C ABI of libherro_b200: FASTQ ingest ->
+//                  hb_upload_reads (or one host read store for all devices) -> feature threads (hb_submit_alignments) fed by the
+//                  alignment stream -> consumer (hb_poll_corrected) -> FASTA, with the time of every stage reported.
 //
 // In the deployed layout these stay in the Rust host; they exist here because no Rust toolchain is available offline and
 // because, once the GPU path runs at hundreds of Mbases/s, single-threaded ingest is the bottleneck (SURVEY.md §8f).
@@ -27,9 +28,12 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <condition_variable>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <deque>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <string_view>
@@ -148,10 +152,13 @@ bool zstd_decompress(const uint8_t* src, size_t n, std::vector<uint8_t>& out) {
         const size_t r = z.decompressStream(ds, &ob, &in);
         produced += ob.pos;
         if (z.isError(r)) { z.freeDStream(ds); t_err = "zstd stream error"; return false; }
-        if (in.pos == in.size && ob.pos < ob.size) break;  // input consumed and the output buffer was not the limit
+        if (in.pos == in.size && (r == 0 || ob.pos < ob.size)) break;  // input consumed, and the last frame ended or the output
+                                                                      // buffer was not the limit
     }
     z.freeDStream(ds);
     out.resize(produced);
+    // a buffer that grew past the text is trimmed: the stream's budget counts the bytes a file holds
+    if (out.capacity() > produced + produced / 16) out.shrink_to_fit();
     return true;
 }
 
@@ -178,6 +185,9 @@ struct hbh_reads {
     uint64_t skipped_short = 0;
 };
 
+struct AlnStream;
+struct hbh_alns_stream;
+
 struct hbh_alns {
     std::vector<std::vector<uint8_t>> text;  // decompressed batch files (the CIGARs point into them)
     std::vector<hb_overlap> ovl;             // grouped by target
@@ -186,6 +196,9 @@ struct hbh_alns {
     double t_decode = 0, t_parse = 0;
     uint64_t lines = 0, kept = 0, compressed_bytes = 0, text_bytes = 0;
     uint32_t files = 0;
+    std::string source;                      // the batch file of a streamed file; empty for a merged load
+    std::shared_ptr<AlnStream> stream;       // the stream whose budget this file holds (NULL for a merged load)
+    uint64_t budget_bytes = 0;               // this file's share of that budget
 };
 
 struct hbh_fasta {
@@ -197,6 +210,7 @@ struct hbh_fasta {
 extern "C" {
 
 const char* hbh_last_error() { return t_err.c_str(); }
+void hbh_alns_free(hbh_alns* a);
 
 // `path`: a FASTQ file (plain or gzip) or a directory holding *.fastq / *.fastq.gz (src/lib.rs:241-265).  core / neighbour:
 // read ids of a cluster file (src/lib.rs:208-239), or NULL / 0 for no filter.
@@ -342,7 +356,6 @@ void hbh_reads_stats(const hbh_reads* r, double* stats4) {
 namespace {
 struct FileAlns {
     std::vector<hb_overlap> ovl;  // in file order
-    std::vector<uint32_t> order;  // target of first appearance order
     uint64_t lines = 0;
     double t_decode = 0, t_parse = 0;
     bool ok = true;
@@ -415,90 +428,304 @@ void parse_batch(const hbh_reads* R, const std::unordered_set<std::string_view>*
         p = le + 1;
     }
 }
-}  // namespace
 
-int hbh_alns_load(const char* dir, const hbh_reads* reads, const char* const* core, uint32_t n_core, int threads, hbh_alns** out) {
-    if (!dir || !reads || !out) return HB_ERR_ARG;
-    *out = nullptr;
-    std::vector<std::string> files;
+// Group a file's overlaps by target, in order of first appearance (the reference's HashMap order is arbitrary, F8), appended to A.
+void group_by_target(const std::vector<hb_overlap>& ovl, hbh_alns& A) {
+    std::unordered_map<uint32_t, uint32_t> slot;
+    std::vector<uint32_t> cnt;
+    std::vector<uint32_t> tids;
+    for (const hb_overlap& o : ovl) {
+        auto it = slot.find(o.tid);
+        if (it == slot.end()) { slot.emplace(o.tid, (uint32_t)cnt.size()); cnt.push_back(1); tids.push_back(o.tid); }
+        else cnt[it->second]++;
+    }
+    if (A.tgt_off.empty()) A.tgt_off.push_back(0);
+    const size_t base = A.ovl.size();
+    std::vector<uint64_t> start(cnt.size() + 1, 0);
+    for (size_t k = 0; k < cnt.size(); k++) start[k + 1] = start[k] + cnt[k];
+    A.ovl.resize(base + ovl.size());
+    std::vector<uint64_t> fill(start.begin(), start.end() - 1);
+    for (const hb_overlap& o : ovl) A.ovl[base + fill[slot[o.tid]]++] = o;
+    for (size_t k = 0; k < cnt.size(); k++) {
+        A.tgt_rid.push_back(tids[k]);
+        A.tgt_off.push_back(base + start[k + 1]);
+    }
+}
+
+bool list_batches(const char* dir, std::vector<std::string>& files) {
     DIR* d = opendir(dir);
-    if (!d) { t_err = std::string("cannot open directory ") + dir; return HB_ERR_ARG; }
+    if (!d) { t_err = std::string("cannot open directory ") + dir; return false; }
     while (dirent* e = readdir(d)) {
         const std::string nme = e->d_name;
         if (nme.size() > 8 && nme.compare(nme.size() - 8, 8, ".oec.zst") == 0) files.push_back(std::string(dir) + "/" + nme);
     }
     closedir(d);
     std::sort(files.begin(), files.end());
+    return true;
+}
+
+uint64_t physical_memory() { return (uint64_t)sysconf(_SC_PHYS_PAGES) * (uint64_t)sysconf(_SC_PAGE_SIZE); }
+
+// The text a batch file will decompress to: the size its first zstd frame records, else four times the file (a guess; the
+// reservation is corrected once the file is decoded).
+uint64_t text_estimate(const std::string& path) {
+    struct stat st;
+    if (stat(path.c_str(), &st) != 0) return 0;
+    uint8_t head[18];
+    const int fd = open(path.c_str(), O_RDONLY);
+    if (fd < 0) return 0;
+    const ssize_t n = pread(fd, head, sizeof head, 0);
+    close(fd);
+    const Zstd& z = zstd();
+    if (n > 0 && z.getFrameContentSize) {
+        const unsigned long long cs = z.getFrameContentSize(head, (size_t)n);
+        if (cs != 0ull - 1 && cs != 0ull - 2) return (uint64_t)cs;
+    }
+    return (uint64_t)st.st_size * 4;
+}
+}  // namespace
+
+// The streaming reader.  Workers take the batch files in sorted name order; a worker starts the next file only while the bytes in
+// flight (decompressed text plus grouped hb_overlap arrays of every file started and not yet freed) are below the budget, or when no
+// file is in flight at all, so one file larger than the budget still runs.  A file decoded early waits in its slot until every
+// earlier file has been handed out.  Starting a file reserves the text it is expected to decompress to (text_estimate), so workers
+// decoding side by side cannot all start at once under the budget; the charge becomes the file's text once decoded, then its text
+// plus its overlap array, and hbh_alns_free releases it.  That may happen after the stream is closed: every streamed hbh_alns keeps
+// the shared state alive.
+struct AlnStream {
+    const hbh_reads* R = nullptr;
+    std::vector<std::string> core_names;          // owned copies: the workers outlive hbh_alns_stream_open's arguments
     std::unordered_set<std::string_view> core_set;
-    if (core) for (uint32_t i = 0; i < n_core; i++) core_set.insert(core[i]);
-    auto* A = new hbh_alns();
-    A->files = (uint32_t)files.size();
-    A->text.resize(files.size());
-    std::vector<FileAlns> per(files.size());
-    std::atomic<uint32_t> next{0};
-    std::atomic<uint64_t> comp{0};
-    auto work = [&]() {
+    bool use_core = false;
+    std::vector<std::string> files;
+    std::vector<uint64_t> estimate;               // text bytes a file is expected to hold, reserved when a worker starts it
+    uint64_t budget = 0;
+    std::mutex mu;
+    std::condition_variable cv;
+    struct Slot { hbh_alns* a = nullptr; bool done = false; std::string err; };
+    std::vector<Slot> slot;
+    size_t next_start = 0, next_out = 0, error_at = SIZE_MAX;
+    uint64_t in_flight = 0, peak = 0;
+    uint32_t files_in_flight = 0, peak_files = 0, parsed = 0;
+    double t_open = 0, t_last_parsed = 0;
+    bool stop = false;
+    std::vector<std::thread> workers;
+
+    void charge(hbh_alns& A, uint64_t bytes) {  // A now holds `bytes` (until now it held A.budget_bytes)
+        std::lock_guard<std::mutex> lk(mu);
+        in_flight = in_flight - A.budget_bytes + bytes;
+        A.budget_bytes = bytes;
+        peak = std::max(peak, in_flight);
+    }
+    void release(const hbh_alns& A) {  // under mu
+        in_flight -= A.budget_bytes;
+        files_in_flight--;
+        cv.notify_all();
+    }
+    static void work(const std::shared_ptr<AlnStream>& sp) {
+        AlnStream& S = *sp;
         for (;;) {
-            const uint32_t i = next.fetch_add(1);
-            if (i >= files.size()) break;
-            FileAlns& fa = per[i];
-            const double t0 = now_s();
-            FileBytes fb;
-            if (!load_file(files[i], fb)) { fa.ok = false; fa.err = t_err; continue; }
-            comp.fetch_add(fb.n);
-            if (!zstd_decompress(fb.p, fb.n, A->text[i])) { fa.ok = false; fa.err = t_err + " in " + files[i]; continue; }
-            fa.t_decode = now_s() - t0;
-            const double t1 = now_s();
-            parse_batch(reads, core ? &core_set : nullptr, A->text[i], fa);
-            fa.t_parse = now_s() - t1;
-        }
-    };
-    std::vector<std::thread> th;
-    for (int i = 0; i < std::max(1, std::min<int>(threads, (int)files.size())); i++) th.emplace_back(work);
-    for (auto& t : th) t.join();
-    // group by target inside every file, in order of first appearance (the reference's HashMap order is arbitrary, F8); a target
-    // named in several files is sent once per file, like the reference's per-batch maps
-    for (size_t i = 0; i < files.size(); i++) {
-        FileAlns& fa = per[i];
-        if (!fa.ok) { t_err = fa.err; delete A; return HB_ERR_INPUT; }
-        A->t_decode += fa.t_decode; A->t_parse += fa.t_parse; A->lines += fa.lines; A->kept += fa.ovl.size();
-        A->text_bytes += A->text[i].size();
-        std::unordered_map<uint32_t, uint32_t> slot;
-        std::vector<uint32_t> cnt;
-        std::vector<uint32_t> tids;
-        for (const hb_overlap& o : fa.ovl) {
-            auto it = slot.find(o.tid);
-            if (it == slot.end()) { slot.emplace(o.tid, (uint32_t)cnt.size()); cnt.push_back(1); tids.push_back(o.tid); }
-            else cnt[it->second]++;
-        }
-        const size_t base = A->ovl.size();
-        std::vector<uint64_t> start(cnt.size() + 1, 0);
-        for (size_t k = 0; k < cnt.size(); k++) start[k + 1] = start[k] + cnt[k];
-        A->ovl.resize(base + fa.ovl.size());
-        std::vector<uint64_t> fill(start.begin(), start.end() - 1);
-        for (const hb_overlap& o : fa.ovl) A->ovl[base + fill[slot[o.tid]]++] = o;
-        for (size_t k = 0; k < cnt.size(); k++) {
-            if (A->tgt_off.empty()) A->tgt_off.push_back(0);
-            A->tgt_rid.push_back(tids[k]);
-            A->tgt_off.push_back(base + start[k + 1]);
+            size_t i;
+            {
+                std::unique_lock<std::mutex> lk(S.mu);
+                S.cv.wait(lk, [&] { return S.stop || S.next_start >= S.files.size() || S.next_start > S.error_at ||
+                                           S.files_in_flight == 0 || S.in_flight < S.budget; });
+                if (S.stop || S.next_start >= S.files.size() || S.next_start > S.error_at) return;
+                i = S.next_start++;
+                S.files_in_flight++;
+                S.peak_files = std::max(S.peak_files, S.files_in_flight);
+                // the reservation keeps the other workers from starting files past the budget while this one decodes
+                S.in_flight += S.estimate[i];
+                S.peak = std::max(S.peak, S.in_flight);
+            }
+            auto* A = new hbh_alns();
+            A->budget_bytes = S.estimate[i];
+            A->files = 1;
+            A->source = S.files[i];
+            A->stream = sp;
+            std::string err;
+            bool ok = false;
+            {
+                const double t0 = now_s();
+                FileBytes fb;
+                A->text.emplace_back();
+                if (!load_file(S.files[i], fb)) {
+                    err = t_err;
+                } else {
+                    A->compressed_bytes = fb.n;
+                    ok = zstd_decompress(fb.p, fb.n, A->text.back());
+                    if (!ok) err = t_err + " in " + S.files[i];
+                }
+                A->t_decode = now_s() - t0;
+            }
+            if (ok) {
+                A->text_bytes = A->text.back().size();
+                S.charge(*A, A->text_bytes);
+                const double t1 = now_s();
+                FileAlns fa;
+                parse_batch(S.R, S.use_core ? &S.core_set : nullptr, A->text.back(), fa);
+                if (fa.ok) {
+                    A->lines = fa.lines;
+                    A->kept = fa.ovl.size();
+                    group_by_target(fa.ovl, *A);
+                    S.charge(*A, A->text_bytes + A->ovl.size() * sizeof(hb_overlap));
+                } else {
+                    ok = false;
+                    err = fa.err + " in " + S.files[i];
+                }
+                A->t_parse = now_s() - t1;
+            }
+            std::unique_lock<std::mutex> lk(S.mu);
+            Slot& sl = S.slot[i];
+            sl.done = true;
+            S.parsed++;
+            S.t_last_parsed = now_s();
+            if (ok) {
+                sl.a = A;
+                S.cv.notify_all();
+            } else {
+                sl.err = err;
+                S.error_at = std::min(S.error_at, i);
+                S.release(*A);
+                A->stream.reset();
+                lk.unlock();
+                delete A;
+            }
         }
     }
-    if (A->tgt_off.empty()) A->tgt_off.push_back(0);
-    A->compressed_bytes = comp.load();
+};
+
+struct hbh_alns_stream { std::shared_ptr<AlnStream> s; };
+
+// Bytes the streaming reader may hold when the caller passes a budget of 0: 1/8 of physical memory.
+uint64_t hbh_alns_default_budget() { return std::max<uint64_t>(physical_memory() / 8, 1); }
+
+// Starts up to `threads` workers that decompress and parse the *.oec.zst files of `dir` ahead of the caller, within `budget_bytes`
+// (0: hbh_alns_default_budget()).  core / n_core as hbh_alns_load.  The caller frees every file hbh_alns_stream_next hands out with
+// hbh_alns_free: files held past the budget stop the workers, so a caller that keeps them all must pass a budget that covers them.
+int hbh_alns_stream_open(const char* dir, const hbh_reads* reads, const char* const* core, uint32_t n_core, int threads,
+                         uint64_t budget_bytes, hbh_alns_stream** out) {
+    if (!dir || !reads || !out) return HB_ERR_ARG;
+    *out = nullptr;
+    auto sp = std::make_shared<AlnStream>();
+    AlnStream& S = *sp;
+    if (!list_batches(dir, S.files)) return HB_ERR_ARG;
+    S.R = reads;
+    if (core) {
+        S.use_core = true;
+        S.core_names.assign(core, core + n_core);
+        for (const std::string& c : S.core_names) S.core_set.insert(c);
+    }
+    S.budget = budget_bytes ? budget_bytes : hbh_alns_default_budget();
+    S.slot.resize(S.files.size());
+    for (const std::string& f : S.files) S.estimate.push_back(text_estimate(f));
+    S.t_open = now_s();
+    S.t_last_parsed = S.t_open;
+    const int n_workers = std::max(1, std::min<int>(threads, (int)S.files.size()));
+    for (int i = 0; i < n_workers && !S.files.empty(); i++) S.workers.emplace_back(AlnStream::work, sp);
+    *out = new hbh_alns_stream{sp};
+    return HB_OK;
+}
+
+// The next file's alignments, in sorted name order: *a is an ordinary hbh_alns (the hbh_alns_* accessors apply), or NULL after the
+// last file.  A file that cannot be read, decompressed or parsed returns HB_ERR_INPUT naming it, here and on every later call.
+int hbh_alns_stream_next(hbh_alns_stream* s, hbh_alns** a) {
+    if (!s || !a) return HB_ERR_ARG;
+    *a = nullptr;
+    AlnStream& S = *s->s;
+    std::unique_lock<std::mutex> lk(S.mu);
+    if (S.next_out >= S.files.size()) return HB_OK;
+    S.cv.wait(lk, [&] { return S.slot[S.next_out].done; });
+    AlnStream::Slot& sl = S.slot[S.next_out];
+    if (!sl.a) { t_err = sl.err; return HB_ERR_INPUT; }
+    *a = sl.a;
+    sl.a = nullptr;
+    S.next_out++;
+    return HB_OK;
+}
+
+// Stops the workers and frees the files not handed out.  Files already handed out stay valid until their hbh_alns_free.
+void hbh_alns_stream_close(hbh_alns_stream* s) {
+    if (!s) return;
+    AlnStream& S = *s->s;
+    {
+        std::lock_guard<std::mutex> lk(S.mu);
+        S.stop = true;
+        S.cv.notify_all();
+    }
+    for (auto& t : S.workers) t.join();
+    std::vector<hbh_alns*> left;
+    {
+        std::lock_guard<std::mutex> lk(S.mu);
+        for (auto& sl : S.slot) if (sl.a) { left.push_back(sl.a); sl.a = nullptr; }
+    }
+    for (hbh_alns* a : left) hbh_alns_free(a);
+    delete s;
+}
+
+// counts6: peak bytes in flight, bytes in flight now, budget, files, files parsed (or failed), peak files in flight.
+// ingest_s: seconds from hbh_alns_stream_open to the last file parsed so far.
+void hbh_alns_stream_stats(hbh_alns_stream* s, uint64_t* counts6, double* ingest_s) {
+    AlnStream& S = *s->s;
+    std::lock_guard<std::mutex> lk(S.mu);
+    if (counts6) {
+        counts6[0] = S.peak; counts6[1] = S.in_flight; counts6[2] = S.budget; counts6[3] = S.files.size(); counts6[4] = S.parsed;
+        counts6[5] = S.peak_files;
+    }
+    if (ingest_s) *ingest_s = S.t_last_parsed - S.t_open;
+}
+
+// Every file of `dir` merged into one hbh_alns: the stream with no budget, its files concatenated in order.  A target named in
+// several files is sent once per file, like the reference's per-batch maps.
+int hbh_alns_load(const char* dir, const hbh_reads* reads, const char* const* core, uint32_t n_core, int threads, hbh_alns** out) {
+    if (!dir || !reads || !out) return HB_ERR_ARG;
+    *out = nullptr;
+    hbh_alns_stream* s = nullptr;
+    int rc = hbh_alns_stream_open(dir, reads, core, n_core, threads, UINT64_MAX, &s);
+    if (rc) return rc;
+    auto* A = new hbh_alns();
+    A->tgt_off.push_back(0);
+    for (;;) {
+        hbh_alns* f = nullptr;
+        rc = hbh_alns_stream_next(s, &f);
+        if (rc) { hbh_alns_stream_close(s); delete A; return rc; }
+        if (!f) break;
+        const uint64_t base = A->ovl.size();
+        A->ovl.insert(A->ovl.end(), f->ovl.begin(), f->ovl.end());
+        A->tgt_rid.insert(A->tgt_rid.end(), f->tgt_rid.begin(), f->tgt_rid.end());
+        for (size_t k = 1; k < f->tgt_off.size(); k++) A->tgt_off.push_back(base + f->tgt_off[k]);
+        for (auto& t : f->text) A->text.push_back(std::move(t));  // the buffers move, so the CIGAR pointers stay valid
+        A->t_decode += f->t_decode; A->t_parse += f->t_parse; A->lines += f->lines; A->kept += f->kept;
+        A->compressed_bytes += f->compressed_bytes; A->text_bytes += f->text_bytes;
+        A->files++;
+        hbh_alns_free(f);
+    }
+    hbh_alns_stream_close(s);
     *out = A;
     return HB_OK;
 }
 
-void hbh_alns_free(hbh_alns* a) { delete a; }
+void hbh_alns_free(hbh_alns* a) {
+    if (!a) return;
+    if (a->stream) {
+        std::lock_guard<std::mutex> lk(a->stream->mu);
+        a->stream->release(*a);
+    }
+    delete a;
+}
 uint32_t hbh_alns_targets(const hbh_alns* a) { return (uint32_t)a->tgt_rid.size(); }
 const uint32_t* hbh_alns_target_rids(const hbh_alns* a) { return a->tgt_rid.data(); }
 const uint64_t* hbh_alns_target_offsets(const hbh_alns* a) { return a->tgt_off.data(); }
 const hb_overlap* hbh_alns_overlaps(const hbh_alns* a) { return a->ovl.data(); }
+// The batch file a streamed hbh_alns came from; "" for hbh_alns_load's merged result.
+const char* hbh_alns_source(const hbh_alns* a) { return a->source.c_str(); }
 // stats6: sum of per-file decode seconds, sum of per-file parse seconds, PAF lines, alignments kept, compressed bytes, text bytes
 void hbh_alns_stats(const hbh_alns* a, double* stats6) {
     stats6[0] = a->t_decode; stats6[1] = a->t_parse; stats6[2] = (double)a->lines; stats6[3] = (double)a->kept;
     stats6[4] = (double)a->compressed_bytes; stats6[5] = (double)a->text_bytes;
 }
+// The bytes a streamed file holds of its stream's budget: its text plus its grouped hb_overlap array.
+uint64_t hbh_alns_budget_bytes(const hbh_alns* a) { return a->budget_bytes; }
 
 // ================================================================================================ FASTA
 int hbh_fasta_open(const char* path, hbh_fasta** out) {
@@ -544,33 +771,43 @@ int hbh_fasta_close(hbh_fasta* w, uint64_t* records, uint64_t* bases) {
 uint64_t hbh_reads_store_bytes(const hbh_reads* r) { return r->woff.back() * 8 + r->qoff.back(); }
 
 // `herro inference --read-alns <alns_dir> -m <model> -b <batch> -t <threads> -d <devices> [-c cluster] <reads> <output>` over the C ABI.
-// devices: n_dev CUDA device ids (targets are dealt to the devices' feature threads from one shared counter, like the
-// reference's per-device worker groups pulling one channel, src/lib.rs:154-187).
+// devices: n_dev CUDA device ids.  The feature threads of every device pull targets from one shared queue that the streaming reader
+// (hbh_alns_stream_*) fills file by file, like the reference's per-device worker groups pulling one channel that alignment_reader
+// fills a batch file at a time (src/lib.rs:154-187, src/overlaps.rs:325-375).  Correction starts once the contexts exist and the
+// first file is parsed, while later files are still being decoded; the feature thread whose hb_submit_alignments returns for a
+// file's last target frees the file (hb_submit_alignments copies the CIGAR bytes), which returns its bytes to the reader's budget.
 // host_store_above: when the packed store is larger than this many bytes, the reads stay in host memory (one hb_read_store that every
 // device attaches; the harness's own packed copy is freed once it exists), else every device gets an uploaded copy.
-// times8: FASTQ load, pack, alignment ingest (wall), read-store upload or host-store creation + attach (max over devices),
-// correction (first submit -> last result), FASTA close, total wall, corrected bases.
+// aln_budget: bytes of decompressed text and hb_overlap arrays the reader may hold at once (0: hbh_alns_default_budget(), 1/8 of
+// physical memory); one file larger than the budget is still read whole.
+// An ingest error (a file that cannot be read or decompressed, a bad header, a malformed line) ends the hand-out of targets at that
+// file: the targets of the files before it are submitted, flushed and their records written, then the call returns HB_ERR_INPUT
+// naming the file.  The output file then holds the records of the targets before the error (the reference panics at that point).
+// times9: FASTQ load, pack, alignment ingest (wall, first file opened -> last file parsed), read-store upload or host-store creation +
+// attach (max over devices), correction (feature threads started -> last result), FASTA close, total wall, corrected bases, first submit
+// (seconds from the start of the call to the first hb_submit_alignments, -1 when there was none).
+// counts6: reads, targets, records, failed targets, peak bytes the alignment reader held, its budget.
 int hbh_inference(const char* reads_path, const char* alns_dir, const char* model, const char* output, uint32_t window, uint32_t batch,
                   int threads, const int* devices, int n_dev, const char* const* core, uint32_t n_core, const char* const* neighbour,
-                  uint32_t n_neigh, int io_threads, uint64_t host_store_above, double* times8, uint64_t* counts4) {
+                  uint32_t n_neigh, int io_threads, uint64_t host_store_above, uint64_t aln_budget, double* times9, uint64_t* counts6) {
     if (!reads_path || !alns_dir || !model || !output || !devices || n_dev < 1) return HB_ERR_ARG;
     const double t_begin = now_s();
     hbh_reads* R = nullptr;
     int rc = hbh_reads_load(reads_path, window, core, n_core, neighbour, n_neigh, io_threads, &R);
     if (rc) return rc;
-    // Context creation (CUDA initialisation, weights) and the read-store upload of every device run while the alignment batches are
-    // decompressed and parsed on the host: the two need nothing from each other (both only read `R`; the alignments need only
+    // Context creation (CUDA initialisation, weights) and the read-store upload of every device run while the first alignment batches
+    // are decompressed and parsed on the host: the two need nothing from each other (both only read `R`; the alignments need only
     // the names and lengths, so the packed words and qualities may go once a host store holds them).
     std::vector<hb_ctx*> ctx((size_t)n_dev, nullptr);
     hb_options opt{};
     opt.struct_size = sizeof opt; opt.window_size = window; opt.batch_size = batch;
     std::vector<double> t_up((size_t)n_dev, 0);
-    hbh_alns* A = nullptr;
+    hbh_alns_stream* S = nullptr;
     hb_read_store* store = nullptr;
     auto cleanup = [&]() {
+        if (S) hbh_alns_stream_close(S);
         for (hb_ctx* c : ctx) if (c) hb_destroy(c);
         if (store) hb_read_store_destroy(store);
-        if (A) hbh_alns_free(A);
         hbh_reads_free(R);
     };
     std::atomic<int> bad{0};
@@ -601,10 +838,8 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
             if (hb_upload_reads(ctx[d], hbh_reads_count(R), hbh_reads_word_ptrs(R), hbh_reads_lens(R), hbh_reads_qual_ptrs(R)) != HB_OK) bad = HB_ERR_CUDA;
             t_up[d] = now_s() - t0;
         });
-    const double t_al0 = now_s();
-    rc = hbh_alns_load(alns_dir, R, core, n_core, io_threads, &A);
-    const double t_ingest = now_s() - t_al0;
-    const std::string ingest_err = rc ? t_err : std::string();
+    rc = hbh_alns_stream_open(alns_dir, R, core, n_core, io_threads, aln_budget, &S);
+    const std::string open_err = rc ? t_err : std::string();
     for (auto& t : dev_th) t.join();
     if (host_store) {
         store_th.join();
@@ -614,7 +849,7 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
             t_up[d] = t_store + now_s() - t0;
         }
     }
-    if (rc) { t_err = ingest_err; cleanup(); return rc; }
+    if (rc) { t_err = open_err; cleanup(); return rc; }
     if (bad.load()) {
         t_err = "context creation / read-store upload failed";
         if (!store_err.empty()) t_err += ": " + store_err;
@@ -626,9 +861,31 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
     hbh_fasta* W = nullptr;
     rc = hbh_fasta_open(output, &W);
     if (rc) { cleanup(); return rc; }
-    const uint32_t n_tgt = hbh_alns_targets(A);
-    std::atomic<uint32_t> next{0};
+    // The shared queue: parsed files in order, each handing out its targets one at a time.  `left` counts the targets of a file not
+    // yet returned from hb_submit_alignments (or abandoned); whoever takes it to zero frees the file.
+    struct QFile {
+        hbh_alns* a;
+        uint32_t n, next;
+        std::atomic<uint32_t> left;
+        QFile(hbh_alns* a_, uint32_t n_) : a(a_), n(n_), next(0), left(n_) {}
+    };
+    std::mutex qmu;
+    std::condition_variable qcv;
+    std::deque<QFile*> queue;
+    bool feed_done = false, abandoned = false;
+    auto done = [](QFile* f, uint32_t k) {
+        if (f->left.fetch_sub(k) == k) { hbh_alns_free(f->a); delete f; }
+    };
+    auto abandon = [&]() {  // under qmu: no further targets are handed out, and the queued files go back to the budget
+        abandoned = true;
+        for (QFile* f : queue) { const uint32_t k = f->n - f->next; f->next = f->n; done(f, k); }
+        queue.clear();
+        qcv.notify_all();
+    };
+    uint64_t n_tgt = 0;
     std::atomic<int> fail{0};
+    std::atomic<bool> submitted{false};
+    double t_first_submit = -1;
     std::atomic<uint64_t> failed_targets{0}, answered{0};
     const double t_c0 = now_s();
     std::vector<std::thread> th;
@@ -639,10 +896,24 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
             th.emplace_back([&, d]() {
                 hb_bind_calling_thread(ctx[d]);
                 for (;;) {
-                    const uint32_t k = next.fetch_add(1);
-                    if (k >= n_tgt || fail.load()) break;
+                    QFile* f;
+                    uint32_t k;
+                    {
+                        std::unique_lock<std::mutex> lk(qmu);
+                        // the timeout only bounds how late a failure set by another thread is noticed
+                        qcv.wait_for(lk, std::chrono::milliseconds(20), [&] { return !queue.empty() || feed_done || abandoned || fail.load(); });
+                        if (fail.load() && !abandoned) abandon();
+                        if (abandoned || (queue.empty() && feed_done)) break;
+                        if (queue.empty()) continue;
+                        f = queue.front();
+                        k = f->next++;
+                        if (f->next == f->n) queue.pop_front();
+                    }
+                    if (!submitted.exchange(true)) t_first_submit = now_s() - t_begin;
+                    const hbh_alns* A = f->a;
                     const uint64_t a0 = A->tgt_off[k], a1 = A->tgt_off[k + 1];
                     const int r = hb_submit_alignments(ctx[d], A->tgt_rid[k], A->ovl.data() + a0, (uint32_t)(a1 - a0));
+                    done(f, 1);
                     if (r == HB_ERR_INPUT) failed_targets.fetch_add(1);   // coordinates the reference would panic on: skip this read
                     else if (r != HB_OK) fail = r;
                 }
@@ -679,21 +950,57 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
             }
         });
     }
+    // This thread feeds the queue from the stream: it blocks while the next file is decoded or the budget is held.
+    int ingest_rc = 0;
+    std::string ingest_err;
+    while (!fail.load()) {
+        hbh_alns* a = nullptr;
+        const int r = hbh_alns_stream_next(S, &a);
+        if (r) { ingest_rc = r; ingest_err = t_err; break; }
+        if (!a) break;
+        const uint32_t n = hbh_alns_targets(a);
+        n_tgt += n;
+        if (n == 0) { hbh_alns_free(a); continue; }
+        std::lock_guard<std::mutex> lk(qmu);
+        if (abandoned) { hbh_alns_free(a); break; }
+        queue.push_back(new QFile(a, n));
+        qcv.notify_all();
+    }
+    {
+        std::lock_guard<std::mutex> lk(qmu);
+        feed_done = true;  // after an ingest error the files before the broken one are still corrected: the hand-out ends there
+        qcv.notify_all();
+    }
+    uint64_t st[6] = {0, 0, 0, 0, 0, 0};
+    double t_ingest = 0;
+    hbh_alns_stream_stats(S, st, &t_ingest);
+    hbh_alns_stream_close(S);
+    S = nullptr;
     for (auto& t : th) t.join();
+    {
+        std::lock_guard<std::mutex> lk(qmu);
+        abandon();  // nothing is left unless every feature thread stopped on a failure
+    }
     const double t_correct = now_s() - t_c0;
     const double t_w0 = now_s();
     uint64_t records = 0, bases = 0;
     hbh_fasta_close(W, &records, &bases);
     const double t_close = now_s() - t_w0;
-    if (times8) {
-        times8[0] = R->t_load; times8[1] = R->t_pack; times8[2] = t_ingest; times8[3] = *std::max_element(t_up.begin(), t_up.end());
-        times8[4] = t_correct; times8[5] = t_close; times8[6] = now_s() - t_begin; times8[7] = (double)bases;
+    if (times9) {
+        times9[0] = R->t_load; times9[1] = R->t_pack; times9[2] = t_ingest; times9[3] = *std::max_element(t_up.begin(), t_up.end());
+        times9[4] = t_correct; times9[5] = t_close; times9[6] = now_s() - t_begin; times9[7] = (double)bases;
+        times9[8] = t_first_submit;
     }
-    if (counts4) { counts4[0] = hbh_reads_count(R); counts4[1] = n_tgt; counts4[2] = records; counts4[3] = failed_targets.load(); }
+    if (counts6) {
+        counts6[0] = hbh_reads_count(R); counts6[1] = n_tgt; counts6[2] = records; counts6[3] = failed_targets.load();
+        counts6[4] = st[0]; counts6[5] = st[2];
+    }
     rc = fail.load();
     if (rc) t_err = std::string("correction failed: ") + hb_last_error(ctx[0]);
+    else if (ingest_rc) { rc = ingest_rc; t_err = ingest_err; }
     cleanup();
     return rc;
 }
 
 }  // extern "C"
+

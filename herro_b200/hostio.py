@@ -40,11 +40,23 @@ def _lib():
         getattr(H, f).restype = vp
     H.hbh_alns_stats.argtypes = [vp, vp]
     H.hbh_alns_stats.restype = None
+    H.hbh_alns_source.argtypes = [vp]
+    H.hbh_alns_source.restype = C.c_char_p
+    H.hbh_alns_budget_bytes.argtypes = [vp]
+    H.hbh_alns_budget_bytes.restype = C.c_uint64
+    H.hbh_alns_default_budget.argtypes = []
+    H.hbh_alns_default_budget.restype = C.c_uint64
+    H.hbh_alns_stream_open.argtypes = [C.c_char_p, vp, vp, u32, C.c_int, C.c_uint64, C.POINTER(vp)]
+    H.hbh_alns_stream_next.argtypes = [vp, C.POINTER(vp)]
+    H.hbh_alns_stream_close.argtypes = [vp]
+    H.hbh_alns_stream_close.restype = None
+    H.hbh_alns_stream_stats.argtypes = [vp, vp, C.POINTER(C.c_double)]
+    H.hbh_alns_stream_stats.restype = None
     H.hbh_fasta_open.argtypes = [C.c_char_p, C.POINTER(vp)]
     H.hbh_fasta_write.argtypes = [vp, C.c_char_p, C.c_char_p, vp, vp, u32]
     H.hbh_fasta_close.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     H.hbh_inference.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, u32, u32, C.c_int, vp, C.c_int, vp, u32, vp, u32,
-                                C.c_int, C.c_uint64, vp, vp]
+                                C.c_int, C.c_uint64, C.c_uint64, vp, vp]
     H.hbh_reads_store_bytes.argtypes = [vp]
     H.hbh_reads_store_bytes.restype = C.c_uint64
     H._io_ready = True
@@ -130,24 +142,50 @@ class Reads:
             pass
 
 
+UNLIMITED = 2 ** 64 - 1  # a budget (bytes) that never holds the alignment reader back
+
+
+def _budget(budget) -> int:
+    """A budget argument -> the reader's: None is the default (1/8 of physical memory), anything else at least one byte."""
+    if budget is None:
+        return 0
+    if int(budget) < 1:
+        raise ValueError(f"the alignment budget must be at least 1 byte, got {budget}")
+    return min(int(budget), UNLIMITED)
+
+
 class Alignments:
-    """overlaps::read_batches + parse_paf (src/overlaps.rs:288-323,117-202), one worker per batch file."""
+    """overlaps::read_batches + parse_paf (src/overlaps.rs:288-323,117-202): every batch file, merged in sorted name order (a target
+    named in several files appears once per file).  `Alignments.stream` yields the files one at a time instead."""
 
     def __init__(self, alns_dir: str, reads: Reads, core=None, threads: int = 0):
         H = _lib()
-        self._H, self._h, self.reads = H, C.c_void_p(), reads
+        h = C.c_void_p()
         ca, nc, self._k = _strs(core)
-        rc = H.hbh_alns_load(alns_dir.encode(), reads._h, ca, nc, threads or min(os.cpu_count() or 1, 32), C.byref(self._h))
+        rc = H.hbh_alns_load(alns_dir.encode(), reads._h, ca, nc, threads or min(os.cpu_count() or 1, 32), C.byref(h))
         if rc != 0:
             raise api.HerroError(rc, H.hbh_last_error().decode())
-        nt = H.hbh_alns_targets(self._h)
+        self._wrap(H, h, reads)
+
+    @classmethod
+    def stream(cls, alns_dir: str, reads: "Reads", core=None, threads: int = 0, budget=None) -> "AlignmentStream":
+        """The batch files one at a time, in sorted name order, while `threads` workers decode the next ones within `budget` bytes
+        of decompressed text and overlap arrays (None: 1/8 of physical memory).  Iterating yields one Alignments per file; close
+        each once its targets are submitted, since files held past the budget stop the workers."""
+        return AlignmentStream(alns_dir, reads, core, threads, budget)
+
+    def _wrap(self, H, h, reads):
+        self._H, self._h, self.reads = H, h, reads
+        nt = H.hbh_alns_targets(h)
         self.n_targets = nt
-        self.target_rids = (np.ctypeslib.as_array(C.cast(H.hbh_alns_target_rids(self._h), C.POINTER(C.c_uint32)), (nt,))
+        self.target_rids = (np.ctypeslib.as_array(C.cast(H.hbh_alns_target_rids(h), C.POINTER(C.c_uint32)), (nt,))
                             if nt else np.zeros(0, np.uint32))
-        self.offsets = np.ctypeslib.as_array(C.cast(H.hbh_alns_target_offsets(self._h), C.POINTER(C.c_uint64)), (nt + 1,))
+        self.offsets = np.ctypeslib.as_array(C.cast(H.hbh_alns_target_offsets(h), C.POINTER(C.c_uint64)), (nt + 1,))
         na = int(self.offsets[-1])
-        buf = (C.c_char * (max(na, 1) * api.OVERLAP_DTYPE.itemsize)).from_address(H.hbh_alns_overlaps(self._h) or 0) if na else None
+        buf = (C.c_char * (max(na, 1) * api.OVERLAP_DTYPE.itemsize)).from_address(H.hbh_alns_overlaps(h) or 0) if na else None
         self.overlaps = np.frombuffer(buf, dtype=api.OVERLAP_DTYPE, count=na) if na else np.zeros(0, api.OVERLAP_DTYPE)
+        self.source = H.hbh_alns_source(h).decode()   # the batch file of a streamed file, "" when merged
+        self.budget_bytes = int(H.hbh_alns_budget_bytes(h))  # what a streamed file holds of its stream's budget
 
     def target(self, k):
         """-> (rid, hb_overlap[] view) of the k-th target group."""
@@ -166,6 +204,67 @@ class Alignments:
         if self._h:
             self._H.hbh_alns_free(self._h)
             self._h = C.c_void_p()
+            self.overlaps = np.zeros(0, api.OVERLAP_DTYPE)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class AlignmentStream:
+    """hbh_alns_stream_*: an iterator of Alignments, one per batch file (see Alignments.stream)."""
+
+    def __init__(self, alns_dir: str, reads: Reads, core=None, threads: int = 0, budget=None):
+        H = _lib()
+        self._H, self._h, self.reads = H, C.c_void_p(), reads
+        ca, nc, self._k = _strs(core)
+        rc = H.hbh_alns_stream_open(alns_dir.encode(), reads._h, ca, nc, threads or min(os.cpu_count() or 1, 32), _budget(budget),
+                                    C.byref(self._h))
+        if rc != 0:
+            raise api.HerroError(rc, H.hbh_last_error().decode())
+
+    def __iter__(self):
+        return self
+
+    def __next__(self) -> Alignments:
+        if not self._h:
+            raise StopIteration
+        h = C.c_void_p()
+        rc = self._H.hbh_alns_stream_next(self._h, C.byref(h))
+        if rc != 0:
+            raise api.HerroError(rc, self._H.hbh_last_error().decode())
+        if not h:
+            raise StopIteration
+        a = Alignments.__new__(Alignments)
+        a._k = None
+        a._wrap(self._H, h, self.reads)
+        return a
+
+    def stats(self) -> dict:
+        c = np.zeros(6, np.uint64)
+        t = C.c_double()
+        self._H.hbh_alns_stream_stats(self._h, c.ctypes.data, C.byref(t))
+        return dict(peak_bytes=int(c[0]), in_flight_bytes=int(c[1]), budget_bytes=int(c[2]), files=int(c[3]), files_parsed=int(c[4]),
+                    peak_files=int(c[5]), ingest_s=t.value)
+
+    def close(self):
+        if self._h:
+            self._H.hbh_alns_stream_close(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
     def __del__(self):
         try:
@@ -353,20 +452,24 @@ def device_bytes(devices) -> list:
 
 
 def inference(reads_path: str, alns_dir: str, model: str, output: str, window: int = 4096, batch: int = 64, threads: int = 1,
-              devices=(0,), core=None, neighbour=None, io_threads: int = 0, read_store=None) -> dict:
+              devices=(0,), core=None, neighbour=None, io_threads: int = 0, read_store=None, aln_buffer_bytes=None) -> dict:
     """The reference's `herro inference --read-alns` command, natively (hbh_inference) -> stage times and counts.  The read store
-    is chosen by host_store_above; read_store ("host" / "device") overrides it."""
+    is chosen by host_store_above; read_store ("host" / "device") overrides it.  The alignment files are decoded while earlier ones
+    are corrected, holding at most aln_buffer_bytes of them (None: 1/8 of physical memory; UNLIMITED: no limit) unless one file is
+    larger on its own.  An alignment file that cannot be read or parsed raises HerroError naming it, after the records of the
+    targets submitted before it have been written."""
     H = _lib()
     dev = np.asarray(list(devices), dtype=np.int32)
     ca, nc, k1 = _strs(core)
     na, nn, k2 = _strs(neighbour)
     above = host_store_above(None if read_store else device_bytes(dev), read_store)
-    t8, c4 = np.zeros(8), np.zeros(4, np.uint64)
+    t9, c6 = np.zeros(9), np.zeros(6, np.uint64)
     rc = H.hbh_inference(reads_path.encode(), alns_dir.encode(), model.encode(), output.encode(), window, batch, threads,
-                         dev.ctypes.data, len(dev), ca, nc, na, nn, io_threads or min(os.cpu_count() or 1, 32), above, t8.ctypes.data,
-                         c4.ctypes.data)
+                         dev.ctypes.data, len(dev), ca, nc, na, nn, io_threads or min(os.cpu_count() or 1, 32), above,
+                         _budget(aln_buffer_bytes), t9.ctypes.data, c6.ctypes.data)
     if rc != 0:
         raise api.HerroError(rc, H.hbh_last_error().decode())
-    return dict(fastq_load_s=t8[0], pack_s=t8[1], alignment_ingest_s=t8[2], read_store_upload_s=t8[3], correction_s=t8[4],
-                fasta_close_s=t8[5], total_s=t8[6], corrected_bases=int(t8[7]), reads=int(c4[0]), targets=int(c4[1]),
-                records=int(c4[2]), failed_targets=int(c4[3]))
+    return dict(fastq_load_s=t9[0], pack_s=t9[1], alignment_ingest_s=t9[2], read_store_upload_s=t9[3], correction_s=t9[4],
+                fasta_close_s=t9[5], total_s=t9[6], corrected_bases=int(t9[7]), first_submit_s=t9[8], reads=int(c6[0]),
+                targets=int(c6[1]), records=int(c6[2]), failed_targets=int(c6[3]), alignment_peak_bytes=int(c6[4]),
+                alignment_budget_bytes=int(c6[5]))
