@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -77,6 +78,10 @@ struct DevBuf {
         cap = ncap;
         return cudaSuccess;
     }
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() const { return (T*)p; }
 };
@@ -84,6 +89,10 @@ struct DevBuf {
 struct PinBuf {
     void* p = nullptr;
     size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() { release(); }
     // grow to hold `bytes`, with 1.5x headroom or exactly; the contents are not kept
     cudaError_t grow(size_t bytes, bool headroom = true) {
         if (bytes <= cap) return cudaSuccess;
@@ -160,6 +169,32 @@ struct HostBatch {
     HostBatch() {}
     explicit HostBatch(int dev) { tgt.dev = win.dev = ovl.dev = ow.dev = cig.dev = dev; }
     void clear() { tgt.clear(); win.clear(); ovl.clear(); ow.clear(); cig.clear(); op_cap = raw_cap = dev_op_cap = 0; n_raw = 0; }
+};
+
+// What every lane owns besides its regions: a stream of its own, events on it and the kernel timer.  hb_create makes them once;
+// they go with the context, after the regions of the lane kind that derives from this (members are destroyed before bases).
+// A launch lane uses all eight events (run_front, launch_tail, hb_replay_last_launch); a single-stage call uses ev[0] for the
+// caller's stream and ev[1] / ev[2] around its device work.
+struct LaneBase {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[8]{};
+    KTimer kt;
+    LaneBase() = default;
+    LaneBase(const LaneBase&) = delete;
+    LaneBase& operator=(const LaneBase&) = delete;
+    ~LaneBase() {
+        for (auto& e : ev) if (e) cudaEventDestroy(e);
+        kt.destroy();
+        if (stream) cudaStreamDestroy(stream);
+    }
+    // The stream and the events; `regions` are then grown in the stream's order.  Returns the error, nullptr on success.
+    const char* create(std::initializer_list<DevBuf*> regions) {
+        if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) return "cudaStreamCreate failed";
+        for (auto& e : ev)
+            if (cudaEventCreate(&e) != cudaSuccess) return "cudaEventCreate failed";
+        for (DevBuf* r : regions) r->st = stream;
+        return nullptr;
+    }
 };
 
 struct Result {
@@ -251,12 +286,9 @@ struct hb_ctx {
     struct ThreadSlot { std::thread::id owner; HostBatch batch; uint32_t handed = 0; /* batches handed over since the last flush */ };
     std::vector<std::unique_ptr<ThreadSlot>> slots;
     PinBuf pin_in;  // staging of hb_upload_reads
-    // Launch lanes (stream + device scratch + pinned result buffers each), one worker thread per lane:
+    // Launch lanes (LaneBase + device scratch + pinned result buffers each), one worker thread per lane:
     // while lane A's worker does its host work (copy-back, per-read reassembly), lane B's batch keeps the GPU busy.
-    struct Lane {
-        cudaStream_t stream = nullptr;
-        cudaEvent_t ev[8]{};
-        KTimer kt;
+    struct Lane : LaneBase {
         // device scratch, one region per moment its size becomes known: the batch (carve_batch), the row arena (carve_rows)
         // and the supported positions (carve_fwd)
         DevBuf d_batch, d_rows, d_fwd;
@@ -269,14 +301,6 @@ struct hb_ctx {
         PinVec<ReadCopy> read_list;
         std::vector<uint32_t> stamp;
         uint32_t stamp_gen = 0;
-        void release() {
-            d_batch.release(); d_rows.release(); d_fwd.release();
-            pin_small.release(); pin_out.release();
-            read_list.release();
-            for (auto& e : ev) if (e) cudaEventDestroy(e);
-            kt.destroy();
-            if (stream) cudaStreamDestroy(stream);
-        }
     };
     // Largest region capacities (and row arena) any lane has needed so far.  A lane that has not run yet (or ran smaller batches)
     // grows its regions to these while it is idle, so that its first real batch allocates nothing (r01: 26 allocations / 226 ms
@@ -290,45 +314,25 @@ struct hb_ctx {
     uint32_t min_launch = 256;  // smallest per-thread hand-over unless launch_targets itself is smaller (HERRO_B200_MIN_LAUNCH: experiments)
     int last_lane = -1;  // lane of the most recently finished launch (debug taps / replay)
     uint32_t chunk_pos = 65536;  // supported positions per forward pass (HERRO_B200_CHUNK_POS): one pass per launch unless huge
-    // hb_forward_batch's lane: its own stream, events, timer and grow-only scratch, which the launch lanes never touch.  Calls
-    // serialise on its mutex.
-    struct FwdLane {
+    // hb_forward_batch's lane: a LaneBase and grow-only scratch of its own, which the launch lanes never touch.  Calls serialise
+    // on its mutex.
+    struct FwdLane : LaneBase {
         std::mutex mu;
-        cudaStream_t stream = nullptr;
-        cudaEvent_t ev[3]{};  // the caller's stream, forward start, forward end
-        KTimer kt;
         PinBuf pin_in, pin_out;     // input region (carve_fwd_in) + the work list; the host outputs
         DevBuf d_in, d_mat, d_fwd;  // input region; the [rows][32] matrices; the forward region (carve_fwd)
-        void release() {
-            d_in.release(); d_mat.release(); d_fwd.release();
-            pin_in.release(); pin_out.release();
-            for (auto& e : ev) if (e) cudaEventDestroy(e);
-            kt.destroy();
-            if (stream) cudaStreamDestroy(stream);
-        }
     } fwd;
     // hb_consensus_batch's lane, shaped like the forward lane, so that a host can run the consensus of one read while the
     // forward of the next one runs.  Calls serialise on its mutex.
-    struct ConsLane {
+    struct ConsLane : LaneBase {
         std::mutex mu;
-        cudaStream_t stream = nullptr;
-        cudaEvent_t ev[3]{};     // the caller's stream, consensus start, consensus end
-        KTimer kt;
         PinBuf pin_in, pin_out;  // input region (carve_cons_in); the emitted lengths and bytes
         DevBuf d_in, d_out;      // input region; the consensus region (carve_cons_out)
         std::vector<uint32_t> order;       // host scratch: key sorting
         std::vector<uint8_t> seq;          // the segments before they are copied out
         std::vector<uint32_t> seg_len;
-        void release() {
-            d_in.release(); d_out.release();
-            pin_in.release(); pin_out.release();
-            for (auto& e : ev) if (e) cudaEventDestroy(e);
-            kt.destroy();
-            if (stream) cudaStreamDestroy(stream);
-        }
     } cons;
-    // hb_features_batch's lane: a launch lane that no worker owns (stream, events, timer, batch and row regions) and never publishes
-    // its sizes to the pipeline's lanes, its own staging batch, and the tables and staging of hb_features_fetch.  Calls of
+    // hb_features_batch's lane: a launch lane that no worker owns (LaneBase, batch and row regions) and never publishes its sizes
+    // to the pipeline's lanes, its own staging batch, and the tables and staging of hb_features_fetch.  Calls of
     // hb_features_batch and hb_features_fetch serialise on its mutex.
     struct FeatLane {
         std::mutex mu;
@@ -338,12 +342,6 @@ struct hb_ctx {
         DevBuf d_tab, d_out;     // the output tables; the host-bound outputs before their copy
         FeatResult res;
         uint64_t ticket = 0;
-        void release() {
-            lane.release();
-            pin_n1.release(); pin_tab.release();
-            d_tab.release(); d_out.release();
-            hbt = HostBatch();
-        }
     } feat;
     bool no_model = false;  // HB_FLAG_NO_MODEL: no weights; the calls that run the forward refuse
 
@@ -844,6 +842,21 @@ void add_forward_flops(const hb_ctx* ctx, hb_stats& S, uint64_t n_sup, const uin
     S.forward_flops += pa;
 }
 
+// T += S for every counter that adds up: all but last_launch_* and the three hb_get_stats computes (host_allocs, ms_host_alloc,
+// ms_submit_wait).  Every call merges its counters through here, under ctx->mu.
+void add_stats(hb_stats& T, const hb_stats& S) {
+    static_assert(offsetof(hb_stats, ms_worker_phase) + sizeof(hb_stats::ms_worker_phase) == sizeof(hb_stats),
+                  "a counter added to hb_stats must be added here too");
+    T.targets += S.targets; T.windows += S.windows; T.overlap_windows += S.overlap_windows; T.rows += S.rows;
+    T.supported += S.supported; T.corrected_bases += S.corrected_bases; T.h2d_bytes += S.h2d_bytes; T.d2h_bytes += S.d2h_bytes;
+    T.kernel_launches += S.kernel_launches; T.device_launches += S.device_launches; T.pileup_algo_bytes += S.pileup_algo_bytes;
+    T.gemm_flops += S.gemm_flops; T.forward_flops += S.forward_flops;
+    T.ms_features += S.ms_features; T.ms_forward += S.ms_forward; T.ms_consensus += S.ms_consensus;
+    T.ms_worker_busy += S.ms_worker_busy; T.ms_worker_gpu_wait += S.ms_worker_gpu_wait;
+    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; T.class_flops[i] += S.class_flops[i]; }
+    for (int i = 0; i < 8; i++) T.ms_worker_phase[i] += S.ms_worker_phase[i];
+}
+
 // The forward + consensus part once the supported positions of every window (nsup[nw]) are known.
 int launch_tail(hb_ctx* ctx, hb_ctx::Lane* L, const BatchView& b, const FwdBufs& f, const uint32_t* nsup, size_t nw, uint64_t* launches) {
     *launches += launch_features_c2(b, L->stream, L->kt);
@@ -1108,16 +1121,9 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         hb_stats& T = ctx->stats;
-        T.ms_worker_busy += S.ms_worker_busy; T.ms_worker_gpu_wait += S.ms_worker_gpu_wait;
         T.last_launch_targets = nt; T.last_launch_windows = nw; T.last_launch_bases = corrected;
-        T.targets += S.targets; T.windows += S.windows; T.overlap_windows += S.overlap_windows; T.rows += S.rows;
-        T.supported += S.supported; T.corrected_bases += S.corrected_bases; T.h2d_bytes += S.h2d_bytes;
-        T.d2h_bytes += S.d2h_bytes; T.kernel_launches += S.kernel_launches; T.device_launches += S.device_launches;
-        T.pileup_algo_bytes += S.pileup_algo_bytes; T.gemm_flops += S.gemm_flops; T.forward_flops += S.forward_flops;
-        T.ms_features += S.ms_features; T.ms_forward += S.ms_forward; T.ms_consensus += S.ms_consensus;
-        for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; T.class_flops[i] += S.class_flops[i]; }
         S.ms_worker_phase[6] = now_ms() - t_mark;
-        for (int i = 0; i < 8; i++) T.ms_worker_phase[i] += S.ms_worker_phase[i];
+        add_stats(T, S);
         for (auto& r : out_results) ctx->results.push_back(std::move(r));
         L->last = std::move(ll);
         ctx->last_lane = (int)(L - ctx->lanes);
@@ -1538,6 +1544,35 @@ int pointer_kind(const void* p, int device) {
     return at.device == device ? 1 : -1;
 }
 
+// One operand of a single-stage call: `may_be_device` operands are memory of the context's device when the call's
+// *_DEVICE_PTRS flag (`dev`, named `flag`) is set and host memory otherwise; every other operand is host memory.  NULL operands
+// are not checked: the calls that take none have rejected them already.
+struct Operand { const char* name; const void* p; bool may_be_device; };
+int check_operands(hb_ctx* ctx, bool dev, const char* flag, std::initializer_list<Operand> ops) {
+    for (const Operand& o : ops) {
+        if (!o.p) continue;
+        const int k = pointer_kind(o.p, ctx->device);
+        if (dev && o.may_be_device && k != 1)
+            return fail(ctx, HB_ERR_ARG, std::string(o.name) + " is not memory of device " + std::to_string(ctx->device) + " (" + flag + " is set)");
+        if ((!dev || !o.may_be_device) && k != 0)
+            return fail(ctx, HB_ERR_ARG, std::string(o.name) + " is device memory" + (o.may_be_device ? std::string(" (") + flag + " is not set)" : ""));
+    }
+    return HB_OK;
+}
+
+// The start of a single-stage call's device work on lane L: its kernel timer armed as hb_set_kernel_timing asks, and with
+// device operands (`dev`) the lane's stream ordered after the work the caller queued on `stream`.
+int stage_begin(hb_ctx* ctx, LaneBase& L, bool dev, void* stream) {
+    L.kt.discard();
+    L.kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
+    L.kt.st = L.stream;
+    if (dev) {
+        CK(cudaEventRecord(L.ev[0], (cudaStream_t)stream));
+        CK(cudaStreamWaitEvent(L.stream, L.ev[0], 0));
+    }
+    return HB_OK;
+}
+
 // The work of hb_forward_batch, with the lane's lock held and the context's device current
 int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,
                   const int32_t* indices, float* info_out, float* logits_out, uint32_t flags, void* stream) {
@@ -1546,18 +1581,9 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     if (B == 0 || Lmax == 0) return fail(ctx, HB_ERR_ARG, "B and Lmax must be positive");
     if (flags & ~HB_FWD_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
     const bool dev = (flags & HB_FWD_DEVICE_PTRS) != 0;
-    {
-        const void* p[6] = {bases, quals, info_out, logits_out, lens, indices};
-        static const char* name[6] = {"bases", "quals", "info_logits", "bases_logits", "lens", "indices"};
-        for (int i = 0; i < 6; i++) {
-            const int k = pointer_kind(p[i], ctx->device);
-            if (dev && i < 4 && k != 1)
-                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is not memory of device " + std::to_string(ctx->device) +
-                                                 " (HB_FWD_DEVICE_PTRS is set)");
-            if ((!dev || i >= 4) && k != 0)
-                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is device memory" + (i < 4 ? " (HB_FWD_DEVICE_PTRS is not set)" : ""));
-        }
-    }
+    int rc = check_operands(ctx, dev, "HB_FWD_DEVICE_PTRS", {{"bases", bases, true}, {"quals", quals, true}, {"info_logits", info_out, true},
+                                                           {"bases_logits", logits_out, true}, {"lens", lens, false}, {"indices", indices, false}});
+    if (rc) return rc;
     uint64_t n = 0;
     uint32_t max_len = 0;
     for (uint32_t b = 0; b < B; b++) {
@@ -1622,13 +1648,8 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     }
     // ---- device work
     KTimer& kt = F.kt;
-    kt.discard();
-    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
-    kt.st = F.stream;
-    if (dev) {
-        CK(cudaEventRecord(F.ev[0], (cudaStream_t)stream));
-        CK(cudaStreamWaitEvent(F.stream, F.ev[0], 0));
-    }
+    rc = stage_begin(ctx, F, dev, stream);
+    if (rc) return rc;
     CK(cudaMemcpyAsync(F.d_in.p, F.pin_in.p, in_sz, cudaMemcpyHostToDevice, F.stream));
     CK(cudaMemcpyAsync(b.fwd_win, h_win, n * 4, cudaMemcpyHostToDevice, F.stream));
     CK(cudaMemcpyAsync(b.fwd_row, h_row, n * 4, cudaMemcpyHostToDevice, F.stream));
@@ -1666,14 +1687,11 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     kt.collect(S.ms_kernel, S.n_kernel);
     kt.on = false;
     add_forward_flops(ctx, S, n, hp.nsup, B);
+    S.ms_forward = ms;
+    S.supported = n;
+    S.kernel_launches = launches;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    hb_stats& T = ctx->stats;
-    T.ms_forward += ms;
-    T.supported += n;
-    T.kernel_launches += launches;
-    T.gemm_flops += S.gemm_flops;
-    T.forward_flops += S.forward_flops;
-    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; T.class_flops[i] += S.class_flops[i]; }
+    add_stats(ctx->stats, S);
     return HB_OK;
 }
 
@@ -1721,18 +1739,11 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
         return fail(ctx, HB_ERR_ARG, "null pointer");
     if (flags & ~HB_CONS_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
     const bool dev = (flags & HB_CONS_DEVICE_PTRS) != 0;
-    {
-        const void* p[10] = {bases, bases_logits, n_windows, rows, n_alns, n_sup, supported, seqs, seg_len, n_segs};
-        static const char* name[10] = {"bases", "bases_logits", "n_windows", "rows", "n_alns", "n_sup", "supported", "seqs", "seg_len", "n_segs"};
-        for (int i = 0; i < 10; i++) {
-            const int k = pointer_kind(p[i], ctx->device);
-            if (dev && i < 2 && k != 1)
-                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is not memory of device " + std::to_string(ctx->device) +
-                                                 " (HB_CONS_DEVICE_PTRS is set)");
-            if ((!dev || i >= 2) && k != 0)
-                return fail(ctx, HB_ERR_ARG, std::string(name[i]) + " is device memory" + (i < 2 ? " (HB_CONS_DEVICE_PTRS is not set)" : ""));
-        }
-    }
+    int rc = check_operands(ctx, dev, "HB_CONS_DEVICE_PTRS",
+                            {{"bases", bases, true}, {"bases_logits", bases_logits, true}, {"n_windows", n_windows, false}, {"rows", rows, false},
+                             {"n_alns", n_alns, false}, {"n_sup", n_sup, false}, {"supported", supported, false}, {"seqs", seqs, false},
+                             {"seg_len", seg_len, false}, {"n_segs", n_segs, false}});
+    if (rc) return rc;
     // ---- sizes and range checks
     uint64_t nw = 0;
     for (uint32_t i = 0; i < n_reads; i++) nw += n_windows[i];
@@ -1814,13 +1825,8 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
     }
     // ---- device work
     KTimer& kt = Cn.kt;
-    kt.discard();
-    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
-    kt.st = Cn.stream;
-    if (dev) {
-        CK(cudaEventRecord(Cn.ev[0], (cudaStream_t)stream));
-        CK(cudaStreamWaitEvent(Cn.stream, Cn.ev[0], 0));
-    }
+    rc = stage_begin(ctx, Cn, dev, stream);
+    if (rc) return rc;
     CK(cudaMemcpyAsync(Cn.d_in.p, Cn.pin_in.p, in_sz, cudaMemcpyHostToDevice, Cn.stream));
     CK(cudaEventRecord(Cn.ev[1], Cn.stream));
     const ConsInArgs ca{dev ? bases : dp.tok, dev ? bases_logits : dp.logits, dp.keys, dp.L, dp.nsel, dp.rowbase, dp.keybase, dp.nkeys,
@@ -1866,11 +1872,10 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
     CK(cudaEventElapsedTime(&ms, Cn.ev[1], Cn.ev[2]));
     kt.collect(S.ms_kernel, S.n_kernel);
     kt.on = false;
+    S.ms_consensus = ms;
+    S.kernel_launches = launches;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    hb_stats& T = ctx->stats;
-    T.ms_consensus += ms;
-    T.kernel_launches += launches;
-    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    add_stats(ctx->stats, S);
     return HB_OK;
 }
 
@@ -1992,13 +1997,12 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
     R.view = b;
     R.valid = true;
     *shape = sh;
+    S.ms_features = ms_front;
+    S.kernel_launches = launches;
+    // run_front times the phases of a launch worker, which this call is not: they stay out of ms_worker_phase
+    std::fill(std::begin(S.ms_worker_phase), std::end(S.ms_worker_phase), 0.0);
     std::lock_guard<std::mutex> lk(ctx->mu);
-    hb_stats& T = ctx->stats;
-    T.ms_features += ms_front;
-    T.kernel_launches += launches;
-    T.h2d_bytes += S.h2d_bytes;
-    T.d2h_bytes += S.d2h_bytes;
-    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    add_stats(ctx->stats, S);
     if (!first_err.empty()) ctx->err = first_err;
     return HB_OK;
 }
@@ -2012,22 +2016,13 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     if (flags & ~HB_FEAT_DEVICE_PTRS) return fail(ctx, HB_ERR_ARG, "unknown flags");
     if (!R.valid || shape->ticket != R.shape.ticket) return fail(ctx, HB_ERR_STATE, "the shape is not the context's latest hb_features_batch result");
     const bool dev = (flags & HB_FEAT_DEVICE_PTRS) != 0;
-    {
-        const void* p[15] = {out->bases, out->quals, out->batch_bases, out->batch_quals, out->status, out->n_windows, out->rows, out->n_alns,
-                             out->n_sup, out->n_ids, out->supported, out->indices, out->ids, out->batch_B, out->batch_Lmax};
-        static const char* name[15] = {"bases", "quals", "batch_bases", "batch_quals", "status", "n_windows", "rows", "n_alns", "n_sup",
-                                       "n_ids", "supported", "indices", "ids", "batch_B", "batch_Lmax"};
-        for (int i = 0; i < 16; i++) {
-            const void* q = i < 15 ? p[i] : out->batch_win;
-            if (!q) continue;
-            const int k = pointer_kind(q, ctx->device);
-            const char* nm = i < 15 ? name[i] : "batch_win";
-            if (dev && i < 4 && k != 1)
-                return fail(ctx, HB_ERR_ARG, std::string(nm) + " is not memory of device " + std::to_string(ctx->device) + " (HB_FEAT_DEVICE_PTRS is set)");
-            if ((!dev || i >= 4) && k != 0)
-                return fail(ctx, HB_ERR_ARG, std::string(nm) + " is device memory" + (i < 4 ? " (HB_FEAT_DEVICE_PTRS is not set)" : ""));
-        }
-    }
+    int rc = check_operands(ctx, dev, "HB_FEAT_DEVICE_PTRS",
+                            {{"bases", out->bases, true}, {"quals", out->quals, true}, {"batch_bases", out->batch_bases, true},
+                             {"batch_quals", out->batch_quals, true}, {"status", out->status, false}, {"n_windows", out->n_windows, false},
+                             {"rows", out->rows, false}, {"n_alns", out->n_alns, false}, {"n_sup", out->n_sup, false}, {"n_ids", out->n_ids, false},
+                             {"supported", out->supported, false}, {"indices", out->indices, false}, {"ids", out->ids, false},
+                             {"batch_B", out->batch_B, false}, {"batch_Lmax", out->batch_Lmax, false}, {"batch_win", out->batch_win, false}});
+    if (rc) return rc;
     const hb_features_shape& sh = R.shape;
     const size_t nt = sh.n_targets, nw = sh.n_windows;
     // ---- the metadata, from the host tables
@@ -2112,21 +2107,16 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     // ---- device work
     hb_ctx::Lane* L = &Fl.lane;
     KTimer& kt = L->kt;
-    kt.discard();
-    kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
-    kt.st = L->stream;
-    if (dev) {
-        CK(cudaEventRecord(L->ev[3], (cudaStream_t)stream));
-        CK(cudaStreamWaitEvent(L->stream, L->ev[3], 0));
-    }
+    rc = stage_begin(ctx, *L, dev, stream);  // the lane's events of the hb_features_batch call were read before it returned
+    if (rc) return rc;
     CK(cudaMemcpyAsync(Fl.d_tab.p, Fl.pin_tab.p, tab_bytes, cudaMemcpyHostToDevice, L->stream));
-    CK(cudaEventRecord(L->ev[4], L->stream));
+    CK(cudaEventRecord(L->ev[1], L->stream));
     uint64_t launches = 0;
     if (o_b || o_q) { kt.begin(K_LISTS); launch_rows_out(d_rows, (uint32_t)n_rseg, b.mat_bases, b.mat_quals, o_b, o_q, L->stream); kt.end(); launches++; }
     if (o_bb || o_bq) { kt.begin(K_LISTS); launch_rows_out(d_batch, (uint32_t)n_bseg, b.mat_bases, b.mat_quals, o_bb, o_bq, L->stream); kt.end(); launches++; }
     if (o_sup || o_idx || o_ids) { kt.begin(K_LISTS); launch_lists_out(b, d_lists, (uint32_t)n_lseg, o_sup, o_idx, o_ids, L->stream); kt.end(); launches++; }
     CK(cudaGetLastError());
-    CK(cudaEventRecord(L->ev[5], L->stream));
+    CK(cudaEventRecord(L->ev[2], L->stream));
     // ---- host-bound outputs straight into the caller's memory
     uint64_t d2h = 0;
     auto copy = [&](void* dst, const void* src, size_t bytes) -> int {
@@ -2135,7 +2125,6 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
         d2h += bytes;
         return HB_OK;
     };
-    int rc = HB_OK;
     if (!dev) {
         if (!rc) rc = copy(out->bases, o_b, sh.n_rows * R_COLS);
         if (!rc) rc = copy(out->quals, o_q, sh.n_rows * R_COLS);
@@ -2150,17 +2139,36 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     // ---- counters
     hb_stats S{};
     float ms = 0;
-    CK(cudaEventElapsedTime(&ms, L->ev[4], L->ev[5]));
+    CK(cudaEventElapsedTime(&ms, L->ev[1], L->ev[2]));
     kt.collect(S.ms_kernel, S.n_kernel);
     kt.on = false;
+    S.ms_features = ms;
+    S.kernel_launches = launches;
+    S.h2d_bytes = tab_bytes;
+    S.d2h_bytes = d2h;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    hb_stats& T = ctx->stats;
-    T.ms_features += ms;
-    T.kernel_launches += launches;
-    T.h2d_bytes += tab_bytes;
-    T.d2h_bytes += d2h;
-    for (int i = 0; i < HB_NUM_KERNEL_CLASSES; i++) { T.ms_kernel[i] += S.ms_kernel[i]; T.n_kernel[i] += S.n_kernel[i]; }
+    add_stats(ctx->stats, S);
     return HB_OK;
+}
+
+// The frame of a single-stage ABI call: the lane's lock `mu` held throughout, the context's device current, and the messages of
+// `body` collected in a string of its own that reaches ctx->err under ctx->mu, since the pipeline's threads share it.
+template <class Body>
+int stage_call(hb_ctx* ctx, std::mutex& mu, Body body) {
+    std::lock_guard<std::mutex> lk(mu);
+    int prev = -1;
+    cudaGetDevice(&prev);
+    std::string err;
+    t_err_sink = &err;
+    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
+    if (rc == HB_OK) rc = body();
+    t_err_sink = nullptr;
+    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
+    if (rc != HB_OK) {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        ctx->err = err;
+    }
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------- read store
@@ -2264,34 +2272,19 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
     ctx->wt.no_fuse_attn = getenv("HERRO_B200_NO_FUSE_ATTN") != nullptr;
     ctx->wt.no_fuse_oproj = getenv("HERRO_B200_NO_FUSE_OPROJ") != nullptr;
     if (!getenv("HERRO_B200_NO_NUMA_BIND")) probe_numa(ctx);
-    for (int li = 0; li < ctx->n_lanes; li++) {
-        auto& L = ctx->lanes[li];
-        if (cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
-        for (auto& e : L.ev)
-            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
-        L.d_batch.st = L.d_rows.st = L.d_fwd.st = L.stream;
-    }
     {
         auto& F = ctx->fwd;
-        if (cudaStreamCreateWithFlags(&F.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
-        for (auto& e : F.ev)
-            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
-        F.d_in.st = F.d_mat.st = F.d_fwd.st = F.stream;
-    }
-    {
         auto& Cn = ctx->cons;
-        if (cudaStreamCreateWithFlags(&Cn.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
-        for (auto& e : Cn.ev)
-            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
-        Cn.d_in.st = Cn.d_out.st = Cn.stream;
-    }
-    {
         auto& Fl = ctx->feat;
-        auto& L = Fl.lane;
-        if (cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return bail(HB_ERR_CUDA); }
-        for (auto& e : L.ev)
-            if (cudaEventCreate(&e) != cudaSuccess) { ctx->err = "cudaEventCreate failed"; return bail(HB_ERR_CUDA); }
-        L.d_batch.st = L.d_rows.st = L.d_fwd.st = Fl.d_tab.st = Fl.d_out.st = L.stream;
+        const char* e = nullptr;
+        for (int li = 0; li < ctx->n_lanes && !e; li++) {
+            auto& L = ctx->lanes[li];
+            e = L.create({&L.d_batch, &L.d_rows, &L.d_fwd});
+        }
+        if (!e) e = F.create({&F.d_in, &F.d_mat, &F.d_fwd});
+        if (!e) e = Cn.create({&Cn.d_in, &Cn.d_out});
+        if (!e) e = Fl.lane.create({&Fl.lane.d_batch, &Fl.lane.d_rows, &Fl.lane.d_fwd, &Fl.d_tab, &Fl.d_out});
+        if (e) { ctx->err = e; return bail(HB_ERR_CUDA); }
         Fl.hbt = HostBatch(cuda_device);
     }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
@@ -2321,23 +2314,15 @@ void hb_destroy(hb_ctx* ctx) {
     ctx->cv_work.notify_all();
     for (auto& L : ctx->lanes) if (L.worker.joinable()) L.worker.join();
     cudaSetDevice(ctx->device);
-    for (auto& L : ctx->lanes) if (L.stream) cudaStreamSynchronize(L.stream);
-    if (ctx->fwd.stream) cudaStreamSynchronize(ctx->fwd.stream);
-    if (ctx->cons.stream) cudaStreamSynchronize(ctx->cons.stream);
-    if (ctx->feat.lane.stream) cudaStreamSynchronize(ctx->feat.lane.stream);
+    std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane};
+    for (auto& L : ctx->lanes) all.push_back(&L);
+    for (LaneBase* L : all) if (L->stream) cudaStreamSynchronize(L->stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
     if (ctx->store) ctx->store->attached.fetch_sub(1);
-    DevBuf* bufs[] = {&ctx->d_words, &ctx->d_word_off, &ctx->d_len, &ctx->d_qual, &ctx->d_qual_off, &ctx->d_ln};
-    for (DevBuf* b : bufs) b->release();
-    for (auto& L : ctx->lanes) L.release();
-    ctx->fwd.release();
-    ctx->cons.release();
-    ctx->feat.release();
-    ctx->pin_in.release();
     ctx->slots.clear();
     ctx->queue.clear();
     ctx->pool.clear();
-    delete ctx;
+    delete ctx;  // the read store's buffers and the lanes release themselves, on the device made current above
 }
 
 int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
@@ -2973,79 +2958,30 @@ int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* base
                      const int32_t* indices, float* info_logits, float* bases_logits, uint32_t flags, void* stream) {
     if (!ctx) return HB_ERR_ARG;
     if (ctx->no_model) return no_model_fail(ctx);
-    std::lock_guard<std::mutex> lk(ctx->fwd.mu);
-    int prev = -1;
-    cudaGetDevice(&prev);
-    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
-    t_err_sink = &err;
-    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
-    if (rc == HB_OK) rc = forward_batch(ctx, B, Lmax, bases, quals, lens, indices, info_logits, bases_logits, flags, stream);
-    t_err_sink = nullptr;
-    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
-    if (rc != HB_OK) {
-        std::lock_guard<std::mutex> g(ctx->mu);
-        ctx->err = err;
-    }
-    return rc;
+    return stage_call(ctx, ctx->fwd.mu, [&] {
+        return forward_batch(ctx, B, Lmax, bases, quals, lens, indices, info_logits, bases_logits, flags, stream);
+    });
 }
 
 int hb_consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, const uint32_t* rows, const uint8_t* n_alns,
                        const uint8_t* bases, const uint32_t* n_sup, const uint32_t* supported, const float* bases_logits, uint8_t* seqs,
                        uint32_t* seg_len, uint32_t* n_segs, uint32_t flags, void* stream) {
     if (!ctx) return HB_ERR_ARG;
-    std::lock_guard<std::mutex> lk(ctx->cons.mu);
-    int prev = -1;
-    cudaGetDevice(&prev);
-    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
-    t_err_sink = &err;
-    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
-    if (rc == HB_OK)
-        rc = consensus_batch(ctx, n_reads, n_windows, rows, n_alns, bases, n_sup, supported, bases_logits, seqs, seg_len, n_segs, flags,
-                             stream);
-    t_err_sink = nullptr;
-    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
-    if (rc != HB_OK) {
-        std::lock_guard<std::mutex> g(ctx->mu);
-        ctx->err = err;
-    }
-    return rc;
+    return stage_call(ctx, ctx->cons.mu, [&] {
+        return consensus_batch(ctx, n_reads, n_windows, rows, n_alns, bases, n_sup, supported, bases_logits, seqs, seg_len, n_segs, flags,
+                               stream);
+    });
 }
 
 int hb_features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const uint32_t* n_ovl, const hb_overlap* ovl,
                       hb_features_shape* shape) {
     if (!ctx) return HB_ERR_ARG;
-    std::lock_guard<std::mutex> lk(ctx->feat.mu);
-    int prev = -1;
-    cudaGetDevice(&prev);
-    std::string err;  // written to ctx->err under the context lock: the pipeline's threads share it
-    t_err_sink = &err;
-    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
-    if (rc == HB_OK) rc = features_batch(ctx, n_targets, rids, n_ovl, ovl, shape);
-    t_err_sink = nullptr;
-    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
-    if (rc != HB_OK) {
-        std::lock_guard<std::mutex> g(ctx->mu);
-        ctx->err = err;
-    }
-    return rc;
+    return stage_call(ctx, ctx->feat.mu, [&] { return features_batch(ctx, n_targets, rids, n_ovl, ovl, shape); });
 }
 
 int hb_features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream) {
     if (!ctx) return HB_ERR_ARG;
-    std::lock_guard<std::mutex> lk(ctx->feat.mu);
-    int prev = -1;
-    cudaGetDevice(&prev);
-    std::string err;
-    t_err_sink = &err;
-    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
-    if (rc == HB_OK) rc = features_fetch(ctx, shape, out, flags, stream);
-    t_err_sink = nullptr;
-    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
-    if (rc != HB_OK) {
-        std::lock_guard<std::mutex> g(ctx->mu);
-        ctx->err = err;
-    }
-    return rc;
+    return stage_call(ctx, ctx->feat.mu, [&] { return features_fetch(ctx, shape, out, flags, stream); });
 }
 
 }  // extern "C"
