@@ -59,6 +59,11 @@ class HbFeaturesShape(C.Structure):
                [(n, C.c_uint64) for n in ("n_rows", "n_sup", "n_ids", "n_batch_rows")]
 
 
+class HbAlignShape(C.Structure):
+    _fields_ = [("ticket", C.c_uint64)] + [(n, C.c_uint32) for n in ("n_overlaps", "n_failed", "n_band_edge")] + \
+               [(n, C.c_uint64) for n in ("cigar_bytes", "cells")] + [("ms_device", C.c_double)]
+
+
 FEATURES_OUT_FIELDS = ("status", "n_windows", "rows", "n_alns", "n_sup", "n_ids", "bases", "quals", "supported", "indices", "ids",
                        "batch_B", "batch_Lmax", "batch_win", "batch_bases", "batch_quals")
 
@@ -124,6 +129,8 @@ def load_library():
     L.hb_consensus_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u32, vp]
     L.hb_features_batch.argtypes = [vp, u32, vp, vp, vp, C.POINTER(HbFeaturesShape)]
     L.hb_features_fetch.argtypes = [vp, C.POINTER(HbFeaturesShape), C.POINTER(HbFeaturesOut), u32, vp]
+    L.hb_align_overlaps.argtypes = [vp, u32, vp, u32, C.POINTER(HbAlignShape)]
+    L.hb_align_fetch.argtypes = [vp, C.POINTER(HbAlignShape), vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -132,10 +139,12 @@ EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "
                     "hb_poll_corrected", "hb_release_result", "hb_last_error", "hb_get_stats", "hb_reset_stats",
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
                     "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch",
-                    "hb_features_batch", "hb_features_fetch", "hb_read_store_create", "hb_read_store_destroy", "hb_attach_read_store"]
+                    "hb_features_batch", "hb_features_fetch", "hb_read_store_create", "hb_read_store_destroy", "hb_attach_read_store",
+                    "hb_align_overlaps", "hb_align_fetch"]
 HB_FWD_DEVICE_PTRS = 1
 HB_CONS_DEVICE_PTRS = 1
 HB_FEAT_DEVICE_PTRS = 1
+HB_ALN_BAND_EDGE = 1
 
 
 def selftest_gemm(M, N, K, act=0, res=0, lda_extra=0, device=0):
@@ -651,6 +660,30 @@ class Context:
         a = {k: v[:size[k]] for k, v in a.items()}
         self.last_features_shape = sh
         return Features([int(r) for r in rids], a, self.batch_size)
+
+    # -- the alignment of overlaps ------------------------------------------------------
+    def align(self, overlaps: np.ndarray, band_w: int = 0) -> dict:
+        """The base-level alignment of overlap-only PAF records (hb_align_overlaps + hb_align_fetch): overlaps is an OVERLAP_DTYPE
+        array whose cigar fields are ignored.  -> dict(overlaps: OVERLAP_DTYPE with the new coordinates and cigar pointers into
+        cigar_text, cigar_text: u8, cigars: list[bytes], status: i32 (HB_OK, HB_ALN_BAND_EDGE or a negative hb_status),
+        matches: u32 (PAF column 10), shape: dict of hb_align_shape).  PAF column 11 is the sum of a CIGAR's op lengths."""
+        if not isinstance(overlaps, np.ndarray) or overlaps.dtype != OVERLAP_DTYPE or overlaps.ndim != 1:
+            raise TypeError("overlaps must be a 1-D OVERLAP_DTYPE array (Context.make_overlaps)")
+        ovl = np.ascontiguousarray(overlaps)
+        n = len(ovl)
+        sh = HbAlignShape()
+        self._check(self._L.hb_align_overlaps(self._h, n, ovl.ctypes.data if n else None, band_w, C.byref(sh)))
+        out = np.zeros(max(n, 1), OVERLAP_DTYPE)
+        text = np.zeros(max(sh.cigar_bytes, 1), np.uint8)
+        status = np.zeros(max(n, 1), np.int32)
+        matches = np.zeros(max(n, 1), np.uint32)
+        self._check(self._L.hb_align_fetch(self._h, C.byref(sh), out.ctypes.data, text.ctypes.data, status.ctypes.data,
+                                           matches.ctypes.data))
+        out, status, matches = out[:n], status[:n], matches[:n]
+        base = text.ctypes.data
+        cigars = [text[int(o["cigar"]) - base:int(o["cigar"]) - base + int(o["cigar_len"])].tobytes() if o["cigar"] else b"" for o in out]
+        shape = {f: getattr(sh, f) for f, _ in HbAlignShape._fields_}
+        return dict(overlaps=out, cigar_text=text, cigars=cigars, status=status, matches=matches, shape=shape)
 
     def set_launch_targets(self, n: int):
         self._check(self._L.hb_set_launch_targets(self._h, n))

@@ -5,6 +5,8 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
     python -m herro_b200.cli inference --torch --read-alns <dir> -d 0 -m model.pt -b 64 reads.fastq out.fasta
                                        (any TorchScript graph with the reference's forward signature, run by torch.jit)
     python -m herro_b200.cli features  --read-alns <dir> reads.fastq out_dir
+    python -m herro_b200.cli align -d 0 [-w 4096] [--band W] [--batch-size 50000] reads.fastq overlaps.paf[.gz] out_dir
+                                       (the CIGARs of an overlap-only PAF aligned on the device, written as --read-alns batches)
     python -m herro_b200.cli predict   -m model.hbw -b 64 [-d 0] features_dir out_dir   (the model alone, on `features` output)
     python -m herro_b200.cli consensus -m model.hbw [-d 0] features_dir logits_dir reads.fastq out.fasta
                                        (consensus alone, on `features` and `predict` output)
@@ -191,6 +193,17 @@ def consensus(args):
     print(f"Wrote {records} records ({bases} bases) to {args.output}.", file=sys.stderr)
 
 
+def align(args):
+    r = hostio.align(args.reads, args.paf, args.output, device=args.device, min_len=args.window_size, band_w=args.band,
+                     batch_size=args.batch_size)
+    print(f"Read {r['lines']} PAF lines ({r['skipped']} skipped: unknown read or self overlap); aligned {r['aligned']}, "
+          f"{r['band_edge']} of them at the band's edge; {r['failed']} failed and not written.", file=sys.stderr)
+    print(f"{r['cells']} DP cells, {r['device_ms'] / 1e3:.2f} s on the device.  Wall time: FASTQ {r['fastq_load_s']:.2f} s, "
+          f"context and upload {r['upload_s']:.2f} s, PAF read {r['paf_read_s']:.2f} s, alignment calls {r['align_s']:.2f} s, "
+          f"formatting and writing {r['write_s']:.2f} s, total {r['total_s']:.2f} s.", file=sys.stderr)
+    return r
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(prog="herro_b200")
     sub = ap.add_subparsers(dest="cmd", required=True)
@@ -215,6 +228,14 @@ def main(argv=None):
     ft.add_argument("--targets-per-launch", type=int, default=256, help="targets per features call")
     ft.add_argument("reads")
     ft.add_argument("output")
+    al = sub.add_parser("align", help="the CIGARs of an overlap-only PAF (minimap2 without -c), written as --read-alns batches")
+    al.add_argument("-d", dest="device", type=int, default=0)
+    al.add_argument("-w", dest="window_size", type=int, default=4096, help="reads shorter than this are not loaded, as in inference")
+    al.add_argument("--band", type=int, default=0, help="band half-width w, a multiple of 16 up to 256 (0: 128)")
+    al.add_argument("--batch-size", type=int, default=50_000, help="reads per output batch file")
+    al.add_argument("reads")
+    al.add_argument("paf")
+    al.add_argument("output")
     pr = sub.add_parser("predict", help="the model alone on a `features` output directory")
     pr.add_argument("-m", dest="model", required=True)
     pr.add_argument("-b", dest="batch_size", type=int, required=True, help="windows per model batch, as `-b` of the features run")
@@ -236,6 +257,8 @@ def main(argv=None):
                 raise SystemExit("-c is not supported with --torch")
             return inference_torch(args)
         return inference(args)
+    if args.cmd == "align":
+        return align(args)
     if args.cmd == "predict":
         return predict(args)
     if args.cmd == "consensus":

@@ -246,6 +246,17 @@ struct FeatResult {
     std::vector<uint32_t> batch_B, batch_Lmax, batch_win;
 };
 
+// What one hb_align_overlaps produced, in the caller's order, until hb_align_fetch copies it out
+struct AlnResult {
+    bool valid = false;
+    hb_align_shape shape{};
+    std::vector<hb_overlap> ovl;  // the input with new coordinates (cigar filled in by hb_align_fetch)
+    std::vector<int32_t> status;
+    std::vector<uint32_t> matches, text_len;
+    std::vector<uint64_t> text_off;
+    std::vector<uint8_t> text;
+};
+
 }  // namespace
 
 // The read store in host memory (hb_read_store_create): every read's words and qualities in one page-locked block that every
@@ -343,6 +354,21 @@ struct hb_ctx {
         FeatResult res;
         uint64_t ticket = 0;
     } feat;
+    // hb_align_overlaps' lane: a LaneBase, the gathered reads of a call (host store), the wave region (jobs, outputs, text offsets,
+    // traceback bytes and op slots) and the CIGAR text of a wave, all grow-only.  Calls of hb_align_overlaps and hb_align_fetch
+    // serialise on its mutex.
+    struct AlnLane : LaneBase {
+        std::mutex mu;
+        DevBuf d_reads, d_wave, d_text;
+        PinBuf pin_jobs, pin_out;  // a wave's jobs and text offsets; its outputs
+        PinVec<ReadCopy> read_list;  // host store: the call's distinct reads, stamped as list_reads does for a launch lane
+        std::vector<uint32_t> stamp;
+        uint32_t stamp_gen = 0;
+        AlnResult res;
+        uint64_t ticket = 0;
+        uint64_t wave_bytes = 8ull << 30;  // traceback bytes and op slots of one wave; HERRO_B200_ALN_WAVE_BYTES: tests shrink it to
+                                           // run several waves
+    } aln;
     bool no_model = false;  // HB_FLAG_NO_MODEL: no weights; the calls that run the forward refuse
 
     std::deque<Result> results;
@@ -663,6 +689,22 @@ struct Carve {
     template <class T> void operator()(T*& p, size_t n) { p = (T*)(base + bytes); bytes += al256(n * sizeof(T)); }
 };
 
+// A host store's gathered reads: the read list, the padded words and qualities and the offset tables, which become `rs`
+void carve_gather(Carve& c, const GatherSizes& gs, ReadsInArgs& g, ReadStoreView& rs) {
+    c(g.list, gs.n_list);
+    c(g.words, READS_FRONT_WORDS + gs.words + READS_BACK_WORDS);
+    c(g.qual, READS_FRONT_QUAL + gs.qual + READS_BACK_QUAL);
+    c(g.word_off, (size_t)gs.n_reads + 1);
+    c(g.qual_off, (size_t)gs.n_reads + 1);
+    g.n = gs.n_list;
+    g.n_words = gs.words;
+    g.n_qual = gs.qual;
+    rs.words = g.words + READS_FRONT_WORDS;
+    rs.word_off = g.word_off;
+    rs.qual = g.qual + READS_FRONT_QUAL;
+    rs.qual_off = g.qual_off;
+}
+
 // Batch region, sized from the HostBatch when a launch starts (the view's n_tgt / n_win / n_ovl / n_ow and W, and the CIGAR
 // bytes and op slots): inputs, raw and tokenised ops, everything per overlap-window, overlap, window and target, counters.  With a
 // host store also the launch's gathered reads, their read list and the offset tables, which become the view's read store.
@@ -712,20 +754,7 @@ size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t r
     c(b.w_outoff, nw);
     c(b.tgt_err, nt);
     c(b.counters, CNT_N);
-    if (gs.n_reads) {
-        c(g.list, gs.n_list);
-        c(g.words, READS_FRONT_WORDS + gs.words + READS_BACK_WORDS);
-        c(g.qual, READS_FRONT_QUAL + gs.qual + READS_BACK_QUAL);
-        c(g.word_off, (size_t)gs.n_reads + 1);
-        c(g.qual_off, (size_t)gs.n_reads + 1);
-        g.n = gs.n_list;
-        g.n_words = gs.words;
-        g.n_qual = gs.qual;
-        b.rs.words = g.words + READS_FRONT_WORDS;
-        b.rs.word_off = g.word_off;
-        b.rs.qual = g.qual + READS_FRONT_QUAL;
-        b.rs.qual_off = g.qual_off;
-    }
+    if (gs.n_reads) carve_gather(c, gs, g, b.rs);
     return c.bytes;
 }
 
@@ -893,28 +922,29 @@ uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw
 #define SYNC_TIMED() do { const double t__ = now_ms(); CK(cudaStreamSynchronize(L->stream)); t_wait += now_ms() - t__; } while (0)
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
 
-// Host store: the distinct reads of a staged batch (its targets and every query), each listed once in L->read_list with its place
-// in the store and in the batch region, reads laid out in order of first appearance.
-int list_reads(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, GatherSizes& gs) {
+// Host store: the distinct reads among the read ids that `each(add)` passes to `add` (at most `n_ids` of them), each listed once
+// in `list` with its place in the store and in the gathered region, reads laid out in order of first appearance.  `stamp` /
+// `stamp_gen` belong to the caller's lane and mark the reads listed so far.
+template <class Each>
+int list_reads(hb_ctx* ctx, PinVec<ReadCopy>& list, std::vector<uint32_t>& stamp, uint32_t& stamp_gen, size_t n_ids, Each each,
+               GatherSizes& gs) {
     const hb_read_store* st = ctx->store;
-    if (L->stamp.size() != st->n_reads) { L->stamp.assign(st->n_reads, 0); L->stamp_gen = 0; }
-    if (++L->stamp_gen == 0) { std::fill(L->stamp.begin(), L->stamp.end(), 0u); L->stamp_gen = 1; }
-    const uint32_t gen = L->stamp_gen;
-    PinVec<ReadCopy>& list = L->read_list;
+    if (stamp.size() != st->n_reads) { stamp.assign(st->n_reads, 0); stamp_gen = 0; }
+    if (++stamp_gen == 0) { std::fill(stamp.begin(), stamp.end(), 0u); stamp_gen = 1; }
+    const uint32_t gen = stamp_gen;
     list.clear();
-    if (!list.reserve(std::min<size_t>(hbt.tgt.size() + hbt.ovl.size(), st->n_reads)))
+    if (!list.reserve(std::min<size_t>(n_ids, st->n_reads)))
         return fail(ctx, HB_ERR_CAPACITY, "out of pinned host memory (read list)");
     uint64_t dw = 0, dq = 0;
     auto add = [&](uint32_t r) {
-        if (L->stamp[r] == gen) return;
-        L->stamp[r] = gen;
+        if (stamp[r] == gen) return;
+        stamp[r] = gen;
         const uint32_t len = st->len[r];
         list.p[list.n++] = ReadCopy{st->word_off[r], st->qual_off[r], dw, dq, r, len};
         dw += ((uint64_t)len + 63) / 64 * 2;
         dq += ((uint64_t)len + 15) / 16 * 16;
     };
-    for (const DevTarget& t : hbt.tgt) add(t.rid);
-    for (const DevOverlap& o : hbt.ovl) add(o.qid);
+    each(add);
     gs = GatherSizes{st->n_reads, (uint32_t)list.size(), dw, dq};
     return HB_OK;
 }
@@ -934,7 +964,10 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
     gs = GatherSizes{};
     g = ReadsInArgs{};
     if (ctx->store) {
-        const int rc = list_reads(ctx, L, hbt, gs);
+        const int rc = list_reads(ctx, L->read_list, L->stamp, L->stamp_gen, hbt.tgt.size() + hbt.ovl.size(), [&](auto& add) {
+            for (const DevTarget& t : hbt.tgt) add(t.rid);
+            for (const DevOverlap& o : hbt.ovl) add(o.qid);
+        }, gs);
         if (rc) return rc;
         g.src_words = ctx->store_words;
         g.src_qual = ctx->store_qual;
@@ -2171,6 +2204,210 @@ int stage_call(hb_ctx* ctx, std::mutex& mu, Body body) {
     return rc;
 }
 
+// ---------------------------------------------------------------------------------- hb_align_overlaps / hb_align_fetch
+constexpr uint32_t ALN_DEFAULT_W = 128;
+
+// The wave region's bytes of one overlap: its (n + 1) x 2w traceback bytes and n + m + 1 op slots
+uint64_t aln_job_bytes(uint64_t n, uint64_t m, uint32_t w) { return al256((n + 1) * 2 * w) + al256((n + m + 1) * 4); }
+
+size_t carve_wave(AlnArgs& a, AlnJob*& jobs, uint64_t*& text_off, size_t nj, uint64_t job_bytes, uint8_t* base) {
+    Carve c{base};
+    c(jobs, nj);
+    c(a.out, nj);
+    c(text_off, nj);
+    c(a.tb, job_bytes);
+    a.jobs = jobs;
+    a.text_off = text_off;
+    return c.bytes;
+}
+
+// The work of hb_align_overlaps, with the lane's lock held and the context's device current
+int align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band_w, hb_align_shape* shape) {
+    hb_ctx::AlnLane& A = ctx->aln;
+    AlnResult& R = A.res;
+    R.valid = false;
+    if (!shape || (n && !ovl)) return fail(ctx, HB_ERR_ARG, "null pointer");
+    const uint32_t w = band_w ? band_w : ALN_DEFAULT_W;
+    if (w % 16 || w > ALN_MAX_W) return fail(ctx, HB_ERR_ARG, "band_w must be 0 (the default) or a multiple of 16 up to 256");
+    if (!ctx->have_reads) return fail(ctx, HB_ERR_STATE, "hb_upload_reads or hb_attach_read_store must be called before hb_align_overlaps");
+    for (uint32_t i = 0; i < n; i++) {
+        if (ovl[i].qid >= ctx->n_reads || ovl[i].tid >= ctx->n_reads) return fail(ctx, HB_ERR_ARG, "overlap " + std::to_string(i) + ": read id out of range");
+        if (ovl[i].strand > 1) return fail(ctx, HB_ERR_ARG, "overlap " + std::to_string(i) + ": strand must be 0 or 1");
+    }
+    // ---- admission: a failed overlap fails alone; the others run longest first
+    R.ovl.assign(ovl, ovl + n);
+    R.status.assign(n, HB_OK);
+    R.matches.assign(n, 0);
+    R.text_off.assign(n, 0);
+    R.text_len.assign(n, 0);
+    R.text.clear();
+    std::vector<uint32_t> order;
+    order.reserve(n);
+    std::string first_err;
+    hb_align_shape sh{};
+    for (uint32_t i = 0; i < n; i++) {
+        const hb_overlap& o = ovl[i];
+        const uint64_t tn = (uint64_t)o.tend - o.tstart, qm = (uint64_t)o.qend - o.qstart;
+        const char* why = nullptr;
+        if (o.qstart > o.qend || o.qend > ctx->read_len[o.qid] || o.tstart > o.tend || o.tend > ctx->read_len[o.tid]) why = "a coordinate lies outside its read";
+        else if (!tn || !qm) why = "an empty span";
+        else if (qm > 2 * tn || tn > 2 * qm) why = "one span more than twice the other";
+        if (why) R.status[i] = HB_ERR_INPUT;
+        else if (aln_job_bytes(tn, qm, w) > A.wave_bytes) { R.status[i] = HB_ERR_CAPACITY; why = "its traceback exceeds the wave region"; }
+        if (why) {
+            sh.n_failed++;
+            if (first_err.empty()) first_err = "overlap " + std::to_string(i) + ": " + why;
+            continue;
+        }
+        order.push_back(i);
+        sh.cells += (tn + 1) * 2 * w;
+    }
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+        return ovl[a].tend - ovl[a].tstart > ovl[b].tend - ovl[b].tstart;
+    });
+    hb_stats S{};
+    double ms_dev = 0;
+    LaneBase& L = A;
+    // ---- the reads: the uploaded store, or the call's reads gathered from the host store
+    ReadStoreView rs = ctx->rs;
+    if (ctx->store && !order.empty()) {
+        GatherSizes gs;
+        ReadsInArgs g{};
+        int rc = list_reads(ctx, A.read_list, A.stamp, A.stamp_gen, 2 * order.size(), [&](auto& add) {
+            for (uint32_t i : order) { add(ovl[i].tid); add(ovl[i].qid); }
+        }, gs);
+        if (rc) return rc;
+        g.src_words = ctx->store_words;
+        g.src_qual = ctx->store_qual;
+        Carve c{nullptr};
+        carve_gather(c, gs, g, rs);
+        CK(A.d_reads.grow(c.bytes));
+        Carve c2{A.d_reads.as<uint8_t>()};
+        carve_gather(c2, gs, g, rs);
+        CK(cudaMemcpyAsync((void*)g.list, A.read_list.data(), vbytes(A.read_list), cudaMemcpyHostToDevice, L.stream));
+        KTimer kt;  // the gather's time is part of the call's, not of a kernel class of hb_stats
+        S.kernel_launches += launch_reads_in(g, L.stream, kt);
+        S.h2d_bytes += vbytes(A.read_list) + gs.words * 8 + gs.qual;
+    }
+    // ---- waves: the next overlaps while their traceback bytes and op slots fit the wave region.  A wave takes at most half of
+    // the device's free memory (what the region already holds counts as free), so that a call beside the pipeline leaves it room;
+    // a wave always holds at least one overlap.
+    size_t mem_free = 0, mem_total = 0;
+    CK(cudaMemGetInfo(&mem_free, &mem_total));
+    const uint64_t budget = std::min<uint64_t>(A.wave_bytes, A.d_wave.cap + mem_free / 2);
+    for (size_t p = 0; p < order.size();) {
+        size_t e = p;
+        uint64_t bytes = 0;
+        while (e < order.size()) {
+            const hb_overlap& o = ovl[order[e]];
+            const uint64_t b = aln_job_bytes(o.tend - o.tstart, o.qend - o.qstart, w);
+            if (e > p && bytes + b > budget) break;
+            bytes += b;
+            e++;
+        }
+        const size_t nj = e - p;
+        AlnArgs a{};
+        a.rs = rs;
+        a.n_jobs = (uint32_t)nj;
+        a.w = w;
+        AlnJob* d_jobs;
+        uint64_t* d_toff;
+        CK(A.d_wave.grow(carve_wave(a, d_jobs, d_toff, nj, bytes, nullptr)));
+        carve_wave(a, d_jobs, d_toff, nj, bytes, A.d_wave.as<uint8_t>());
+        CK(A.pin_jobs.grow(nj * (sizeof(AlnJob) + 8)));
+        CK(A.pin_out.grow(nj * sizeof(AlnOut)));
+        AlnJob* jobs = A.pin_jobs.as<AlnJob>();
+        uint64_t* toff = (uint64_t*)(jobs + nj);
+        uint64_t off = 0;
+        for (size_t k = 0; k < nj; k++) {
+            const uint32_t i = order[p + k];
+            const hb_overlap& o = ovl[i];
+            const uint64_t tn = o.tend - o.tstart, qm = o.qend - o.qstart;
+            jobs[k] = AlnJob{o.qid, o.tid, o.strand, i, o.qstart, o.qend, o.tstart, o.tend, off, 0};
+            off += al256((tn + 1) * 2 * w);
+            jobs[k].op_off = off / 4;  // the op slots follow the traceback bytes (both 256-byte aligned)
+            off += al256((tn + qm + 1) * 4);
+        }
+        a.ops = (uint32_t*)a.tb;
+        CK(cudaMemcpyAsync(d_jobs, jobs, nj * sizeof(AlnJob), cudaMemcpyHostToDevice, L.stream));
+        CK(cudaEventRecord(L.ev[1], L.stream));
+        launch_align_fill(a, L.stream);
+        launch_align_trace(a, L.stream);
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(L.ev[2], L.stream));
+        AlnOut* out = A.pin_out.as<AlnOut>();
+        CK(cudaMemcpyAsync(out, a.out, nj * sizeof(AlnOut), cudaMemcpyDeviceToHost, L.stream));
+        CK(cudaStreamSynchronize(L.stream));
+        float ms = 0;
+        CK(cudaEventElapsedTime(&ms, L.ev[1], L.ev[2]));
+        ms_dev += ms;
+        S.kernel_launches += 2;
+        S.h2d_bytes += nj * sizeof(AlnJob);
+        S.d2h_bytes += nj * sizeof(AlnOut);
+        // ---- the text: placed by a scan of the text lengths, written on the device, copied out
+        const uint64_t t0 = R.text.size();
+        uint64_t tb = 0;
+        for (size_t k = 0; k < nj; k++) {
+            if (out[k].edge > 1) return fail(ctx, HB_ERR_CUDA, "overlap " + std::to_string(jobs[k].idx) + ": traceback left the band (internal error)");
+            toff[k] = tb;
+            tb += out[k].text_len;
+            const uint32_t i = jobs[k].idx;
+            hb_overlap& r = R.ovl[i];
+            r.qstart = out[k].qstart; r.qend = out[k].qend; r.tstart = out[k].tstart; r.tend = out[k].tend;
+            R.status[i] = out[k].edge ? HB_ALN_BAND_EDGE : HB_OK;
+            sh.n_band_edge += out[k].edge ? 1 : 0;
+            R.matches[i] = out[k].matches;
+            R.text_off[i] = t0 + toff[k];
+            R.text_len[i] = out[k].text_len;
+        }
+        CK(A.d_text.grow(std::max<uint64_t>(tb, 1)));
+        a.text = A.d_text.as<uint8_t>();
+        R.text.resize(t0 + tb);
+        CK(cudaMemcpyAsync(d_toff, toff, nj * 8, cudaMemcpyHostToDevice, L.stream));
+        CK(cudaEventRecord(L.ev[1], L.stream));
+        launch_align_text(a, L.stream);
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(L.ev[2], L.stream));
+        if (tb) CK(cudaMemcpyAsync(R.text.data() + t0, a.text, tb, cudaMemcpyDeviceToHost, L.stream));
+        CK(cudaStreamSynchronize(L.stream));
+        CK(cudaEventElapsedTime(&ms, L.ev[1], L.ev[2]));
+        ms_dev += ms;
+        S.kernel_launches += 1;
+        S.h2d_bytes += nj * 8;
+        S.d2h_bytes += tb;
+        p = e;
+    }
+    sh.ticket = ++A.ticket;
+    sh.n_overlaps = n;
+    sh.cigar_bytes = R.text.size();
+    sh.ms_device = ms_dev;
+    R.shape = sh;
+    R.valid = true;
+    *shape = sh;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    add_stats(ctx->stats, S);
+    if (!first_err.empty()) ctx->err = first_err;
+    return HB_OK;
+}
+
+// The work of hb_align_fetch, with the lane's lock held
+int align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8_t* cigar_text, int32_t* status, uint32_t* matches) {
+    const AlnResult& R = ctx->aln.res;
+    if (!shape) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (!R.valid || shape->ticket != R.shape.ticket) return fail(ctx, HB_ERR_STATE, "the shape is not the context's latest hb_align_overlaps result");
+    const size_t n = R.shape.n_overlaps;
+    if (cigar_text && !R.text.empty()) memcpy(cigar_text, R.text.data(), R.text.size());
+    if (status && n) memcpy(status, R.status.data(), n * 4);
+    if (matches && n) memcpy(matches, R.matches.data(), n * 4);
+    if (out)
+        for (size_t i = 0; i < n; i++) {
+            out[i] = R.ovl[i];
+            out[i].cigar = cigar_text && R.text_len[i] ? cigar_text + R.text_off[i] : nullptr;
+            out[i].cigar_len = R.text_len[i];
+        }
+    return HB_OK;
+}
+
 // ---------------------------------------------------------------------------------- read store
 // ln(k) table from the host libm — the value Rust's f64::ln returns (src/features.rs:507)
 int upload_ln_table(hb_ctx* ctx, uint32_t max_len) {
@@ -2267,6 +2504,7 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
     ctx->pileup_v1 = getenv("HERRO_B200_PILEUP_V1") != nullptr;
     ctx->host_windowing = getenv("HERRO_B200_HOST_WINDOWING") != nullptr;
     if (const char* e = getenv("HERRO_B200_ARENA_ROWS")) ctx->arena_rows_per_win = (uint32_t)std::max(atoi(e), 1);
+    if (const char* e = getenv("HERRO_B200_ALN_WAVE_BYTES")) ctx->aln.wave_bytes = std::max<uint64_t>(strtoull(e, nullptr, 10), 1);
     ctx->wt.no_fuse_ln = getenv("HERRO_B200_NO_FUSE_LN") != nullptr;
     ctx->wt.no_fuse_ffn = getenv("HERRO_B200_NO_FUSE_FFN") != nullptr;
     ctx->wt.no_fuse_attn = getenv("HERRO_B200_NO_FUSE_ATTN") != nullptr;
@@ -2284,6 +2522,7 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         if (!e) e = F.create({&F.d_in, &F.d_mat, &F.d_fwd});
         if (!e) e = Cn.create({&Cn.d_in, &Cn.d_out});
         if (!e) e = Fl.lane.create({&Fl.lane.d_batch, &Fl.lane.d_rows, &Fl.lane.d_fwd, &Fl.d_tab, &Fl.d_out});
+        if (!e) e = ctx->aln.create({&ctx->aln.d_reads, &ctx->aln.d_wave, &ctx->aln.d_text});
         if (e) { ctx->err = e; return bail(HB_ERR_CUDA); }
         Fl.hbt = HostBatch(cuda_device);
     }
@@ -2314,7 +2553,7 @@ void hb_destroy(hb_ctx* ctx) {
     ctx->cv_work.notify_all();
     for (auto& L : ctx->lanes) if (L.worker.joinable()) L.worker.join();
     cudaSetDevice(ctx->device);
-    std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane};
+    std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane, &ctx->aln};
     for (auto& L : ctx->lanes) all.push_back(&L);
     for (LaneBase* L : all) if (L->stream) cudaStreamSynchronize(L->stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
@@ -2982,6 +3221,16 @@ int hb_features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, con
 int hb_features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream) {
     if (!ctx) return HB_ERR_ARG;
     return stage_call(ctx, ctx->feat.mu, [&] { return features_fetch(ctx, shape, out, flags, stream); });
+}
+
+int hb_align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band_w, hb_align_shape* shape) {
+    if (!ctx) return HB_ERR_ARG;
+    return stage_call(ctx, ctx->aln.mu, [&] { return align_overlaps(ctx, n, ovl, band_w, shape); });
+}
+
+int hb_align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8_t* cigar_text, int32_t* status, uint32_t* matches) {
+    if (!ctx) return HB_ERR_ARG;
+    return stage_call(ctx, ctx->aln.mu, [&] { return align_fetch(ctx, shape, out, cigar_text, status, matches); });
 }
 
 }  // extern "C"

@@ -237,4 +237,31 @@ int launch_features_c1(const BatchView& b, cudaStream_t st, KTimer& kt);
 int launch_features_c2(const BatchView& b, cudaStream_t st, KTimer& kt);
 int launch_consensus(const BatchView& b, cudaStream_t st, KTimer& kt);
 
+// align.cu: hb_align_overlaps.  One job per overlap of a wave: the target slice [tstart, tend) of read tid and the query slice
+// [qstart, qend) of read qid (reverse-complemented on strand 1); its traceback bytes at tb + tb_off ((n + 1) x 2w) and its op
+// slots at ops + op_off (n + m + 1).
+constexpr uint32_t ALN_MAX_W = 256;  // band half-width: 2w cells per row, at most 16 per lane
+struct AlnJob {
+    uint32_t qid, tid, strand, idx;  // idx: the overlap's place in the call
+    uint32_t qstart, qend, tstart, tend;
+    uint64_t tb_off, op_off;
+};
+struct AlnOut {  // per job: new coordinates, edge (1: the path touched the band's edge; 2: internal error), the counts
+    uint32_t qstart, qend, tstart, tend;
+    uint32_t edge, matches, n_ops, text_len;
+};
+struct AlnArgs {
+    ReadStoreView rs;
+    const AlnJob* jobs;
+    uint32_t n_jobs, w;
+    uint8_t* tb;
+    uint32_t* ops;
+    AlnOut* out;
+    const uint64_t* text_off;  // k_align_text: each job's text at text + text_off[job]
+    uint8_t* text;
+};
+void launch_align_fill(const AlnArgs& a, cudaStream_t st);
+void launch_align_trace(const AlnArgs& a, cudaStream_t st);
+void launch_align_text(const AlnArgs& a, cudaStream_t st);
+
 }  // namespace hb

@@ -10,6 +10,11 @@
 //                  other on one thread; here workers decompress (libzstd through dlopen: the image ships the library but no
 //                  header) and parse upcoming files while earlier ones are used (hbh_alns_stream_*), within a budget of host
 //                  memory; hbh_alns_load is the same stream with no budget, merged.
+//   hbh_paf_*      an overlap-only PAF (plain or .gz, minimap2 without -c), read in chunks of lines under parse_paf's admission
+//                  rules: unknown read names and self overlaps skipped, any cg:Z: ignored, repeated pairs kept
+//   hbh_batches_*  the write mode of generate_batches (src/overlaps.rs:264-285, scripts/batch.py): <k>.oec.zst holds the k-th run of
+//                  batch_size loaded reads (header: the count, then one id per line) and every line whose target is among them
+//   hbh_align      `herro align`: hbh_paf_* -> hb_align_overlaps -> hbh_batches_*
 //   hbh_fasta_*    correction_writer / write_sequence (src/lib.rs:267-317): `>id[:k] description\n seq\n`
 //   hbh_inference  the whole `herro inference --read-alns` pipeline over the public C ABI of libherro_b200: FASTQ ingest ->
 //                  hb_upload_reads (or one host read store for all devices) -> feature threads (hb_submit_alignments) fed by the
@@ -110,7 +115,11 @@ struct Zstd {
     size_t (*decompressStream)(void*, ZOutBuf*, ZInBuf*) = nullptr;
     unsigned (*isError)(size_t) = nullptr;
     unsigned long long (*getFrameContentSize)(const void*, size_t) = nullptr;
+    void* (*createCCtx)() = nullptr;
+    size_t (*freeCCtx)(void*) = nullptr;
+    size_t (*compressStream2)(void*, ZOutBuf*, ZInBuf*, int) = nullptr;  // ZSTD_e_continue 0, ZSTD_e_end 2
     bool ok = false;
+    bool ok_c = false;
 };
 const Zstd& zstd() {
     static Zstd z = [] {
@@ -126,7 +135,11 @@ const Zstd& zstd() {
         r.decompressStream = (size_t(*)(void*, ZOutBuf*, ZInBuf*))dlsym(r.h, "ZSTD_decompressStream");
         r.isError = (unsigned (*)(size_t))dlsym(r.h, "ZSTD_isError");
         r.getFrameContentSize = (unsigned long long (*)(const void*, size_t))dlsym(r.h, "ZSTD_getFrameContentSize");
+        r.createCCtx = (void* (*)())dlsym(r.h, "ZSTD_createCCtx");
+        r.freeCCtx = (size_t(*)(void*))dlsym(r.h, "ZSTD_freeCCtx");
+        r.compressStream2 = (size_t(*)(void*, ZOutBuf*, ZInBuf*, int))dlsym(r.h, "ZSTD_compressStream2");
         r.ok = r.createDStream && r.freeDStream && r.initDStream && r.decompressStream && r.isError;
+        r.ok_c = r.createCCtx && r.freeCCtx && r.compressStream2 && r.isError;
         return r;
     }();
     return z;
@@ -1004,3 +1017,288 @@ int hbh_inference(const char* reads_path, const char* alns_dir, const char* mode
 
 }  // extern "C"
 
+// ================================================================================================ overlap-only PAF -> aligned batches
+struct hbh_paf {
+    gzFile g = nullptr;               // gzopen reads plain files as they are
+    std::vector<uint8_t> buf;         // the current chunk's lines (the admitted lines' mapq fields lie in it)
+    size_t carry = 0;                 // bytes of an unfinished line kept from the previous read
+    bool eof = false;
+    const hbh_reads* R = nullptr;
+    std::vector<hb_overlap> ovl;      // the admitted lines of the current chunk, cigar NULL
+    std::vector<std::pair<uint32_t, uint32_t>> mapq;  // column 12 of each admitted line: offset into buf, length
+    uint64_t lines = 0, skipped = 0, bytes = 0;
+};
+
+struct hbh_batches {
+    struct File { FILE* f = nullptr; void* cctx = nullptr; std::string pending; uint64_t lines = 0; };
+    std::vector<File> files;
+    const hbh_reads* R = nullptr;
+    uint32_t batch_size = 0;
+    std::vector<uint8_t> zbuf;
+    uint64_t written = 0;
+};
+
+namespace {
+
+constexpr size_t PAF_READ = 16u << 20;
+
+bool flush_batch(hbh_batches* B, hbh_batches::File& F, bool end) {
+    const Zstd& z = zstd();
+    ZInBuf in{F.pending.data(), F.pending.size(), 0};
+    for (;;) {
+        ZOutBuf out{B->zbuf.data(), B->zbuf.size(), 0};
+        const size_t r = z.compressStream2(F.cctx, &out, &in, end ? 2 : 0);
+        if (z.isError(r)) { t_err = "zstd compression failed"; return false; }
+        if (out.pos && fwrite(B->zbuf.data(), 1, out.pos, F.f) != out.pos) { t_err = "write failed"; return false; }
+        if (end ? r == 0 : in.pos == in.size) break;
+    }
+    F.pending.clear();
+    return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hbh_batches_close(hbh_batches* B, uint64_t* lines_per_batch);
+
+// An overlap-only PAF (plain or gzip).  Lines are admitted as parse_paf admits them (src/overlaps.rs:117-202) with reads' names
+// (reads shorter than the window are not loaded, so their lines go), self overlaps skipped; a cg:Z: field is ignored.
+int hbh_paf_open(const char* path, const hbh_reads* reads, hbh_paf** out) {
+    if (!path || !reads || !out) { t_err = "null pointer"; return HB_ERR_ARG; }
+    gzFile g = gzopen(path, "rb");
+    if (!g) { t_err = std::string("cannot open ") + path; return HB_ERR_INPUT; }
+    gzbuffer(g, 1 << 20);
+    hbh_paf* P = new hbh_paf;
+    P->g = g;
+    P->R = reads;
+    *out = P;
+    return HB_OK;
+}
+
+// The next chunk: up to max_lines admitted lines (fewer at the end of the file; 0 once it is read).  *n_out is their count; their
+// overlaps (hbh_paf_overlaps) stay valid until the next call.
+int hbh_paf_next(hbh_paf* P, uint32_t max_lines, uint32_t* n_out) {
+    if (!P || !n_out || !max_lines) { t_err = "null pointer or zero max_lines"; return HB_ERR_ARG; }
+    P->ovl.clear();
+    P->mapq.clear();
+    *n_out = 0;
+    // keep reading until max_lines are admitted or the file ends; the unparsed tail of the buffer carries over
+    std::vector<uint8_t>& b = P->buf;
+    size_t pos = 0;
+    if (P->carry) { memmove(b.data(), b.data() + b.size() - P->carry, P->carry); b.resize(P->carry); P->carry = 0; }
+    else b.clear();
+    while (P->ovl.size() < max_lines) {
+        const uint8_t* base = b.data();
+        const uint8_t* e = base + b.size();
+        const uint8_t* p = base + pos;
+        const uint8_t* nl = (const uint8_t*)memchr(p, '\n', (size_t)(e - p));
+        if (!nl) {
+            if (P->eof) {
+                if (p == e) break;
+                b.push_back('\n');  // a last line without a newline
+                continue;
+            }
+            const size_t old = b.size();
+            b.resize(old + PAF_READ);
+            const int r = gzread(P->g, b.data() + old, (unsigned)PAF_READ);
+            if (r < 0) { t_err = "PAF read error"; return HB_ERR_INPUT; }
+            b.resize(old + (size_t)r);
+            P->bytes += (uint64_t)r;
+            if (r == 0) P->eof = true;
+            continue;
+        }
+        pos = (size_t)(nl + 1 - base);
+        const uint8_t* le = nl;
+        if (le > p && le[-1] == '\r') le--;
+        if (le == p) continue;
+        P->lines++;
+        const uint8_t* f[12][2];
+        int nf = 0;
+        for (const uint8_t* c = p; nf < 12;) {
+            const uint8_t* t = (const uint8_t*)memchr(c, '\t', (size_t)(le - c));
+            if (!t) t = le;
+            f[nf][0] = c; f[nf][1] = t;
+            nf++;
+            if (t == le) break;
+            c = t + 1;
+        }
+        if (nf < 12) { t_err = "PAF line " + std::to_string(P->lines) + ": fewer than 12 columns"; return HB_ERR_INPUT; }
+        auto qit = P->R->name_to_id.find(std::string_view((const char*)f[0][0], (size_t)(f[0][1] - f[0][0])));
+        auto tit = P->R->name_to_id.find(std::string_view((const char*)f[5][0], (size_t)(f[5][1] - f[5][0])));
+        if (qit == P->R->name_to_id.end() || tit == P->R->name_to_id.end() || qit->second == tit->second) { P->skipped++; continue; }
+        hb_overlap o{};
+        o.qid = qit->second;
+        o.tid = tit->second;
+        const uint8_t sc = f[4][0] < f[4][1] ? *f[4][0] : 0;
+        if (!parse_u32(f[1][0], f[1][1], o.qlen) || !parse_u32(f[2][0], f[2][1], o.qstart) || !parse_u32(f[3][0], f[3][1], o.qend) ||
+            !parse_u32(f[6][0], f[6][1], o.tlen) || !parse_u32(f[7][0], f[7][1], o.tstart) || !parse_u32(f[8][0], f[8][1], o.tend) ||
+            (sc != '+' && sc != '-')) {
+            t_err = "PAF line " + std::to_string(P->lines) + ": malformed number or strand";
+            return HB_ERR_INPUT;
+        }
+        o.strand = sc == '-';
+        P->ovl.push_back(o);
+        P->mapq.emplace_back((uint32_t)(f[11][0] - base), (uint32_t)(f[11][1] - f[11][0]));
+    }
+    // the unparsed rest carries over to the next call
+    P->carry = b.size() - pos;
+    *n_out = (uint32_t)P->ovl.size();
+    return HB_OK;
+}
+
+const hb_overlap* hbh_paf_overlaps(const hbh_paf* P) { return P->ovl.data(); }
+void hbh_paf_stats(const hbh_paf* P, uint64_t* counts3) { counts3[0] = P->lines; counts3[1] = P->skipped; counts3[2] = P->bytes; }
+void hbh_paf_close(hbh_paf* P) {
+    if (!P) return;
+    if (P->g) gzclose(P->g);
+    delete P;
+}
+
+// <dir>/<k>.oec.zst for k < ceil(reads / batch_size), each starting with its header
+int hbh_batches_open(const char* dir, const hbh_reads* reads, uint32_t batch_size, hbh_batches** out) {
+    if (!dir || !reads || !out || !batch_size) { t_err = "null pointer or zero batch size"; return HB_ERR_ARG; }
+    if (!zstd().ok_c) { t_err = "libzstd with ZSTD_compressStream2 not found"; return HB_ERR_STATE; }
+    mkdir(dir, 0777);
+    hbh_batches* B = new hbh_batches;
+    B->R = reads;
+    B->batch_size = batch_size;
+    B->zbuf.resize(1 << 17);
+    const uint32_t n = (uint32_t)reads->id.size();
+    for (uint32_t k = 0; (uint64_t)k * batch_size < n; k++) {
+        hbh_batches::File F;
+        const std::string path = std::string(dir) + "/" + std::to_string(k) + ".oec.zst";
+        F.f = fopen(path.c_str(), "wb");
+        F.cctx = zstd().createCCtx();
+        const uint32_t r0 = k * batch_size, r1 = std::min<uint64_t>((uint64_t)r0 + batch_size, n);
+        F.pending = std::to_string(r1 - r0) + "\n";
+        for (uint32_t r = r0; r < r1; r++) { F.pending += reads->id[r]; F.pending += '\n'; }
+        const bool ok = F.f && F.cctx;
+        B->files.push_back(std::move(F));
+        if (!ok) { t_err = "cannot create " + path; hbh_batches_close(B, nullptr); return HB_ERR_INPUT; }
+    }
+    *out = B;
+    return HB_OK;
+}
+
+// Append the lines of one chunk: line i of `paf`'s current chunk with the coordinates and CIGAR of aligned[i] (hb_align_fetch's
+// `out`), matches[i] as column 10 and the sum of the CIGAR's op lengths as column 11, to the batch of its target, in input order.
+// Lines with status[i] < 0 are not written.
+int hbh_batches_write(hbh_batches* B, const hbh_paf* paf, const hb_overlap* aligned, const int32_t* status, const uint32_t* matches,
+                      uint32_t n) {
+    if (!B || !paf || (n && (!aligned || !status || !matches)) || n > paf->ovl.size()) { t_err = "bad arguments"; return HB_ERR_ARG; }
+    const hbh_reads* R = B->R;
+    for (uint32_t i = 0; i < n; i++) {
+        if (status[i] < 0) continue;
+        const hb_overlap& o = aligned[i];
+        uint64_t block = 0, v = 0;
+        for (uint32_t c = 0; c < o.cigar_len; c++) {
+            const uint8_t ch = o.cigar[c];
+            if (ch >= '0' && ch <= '9') v = v * 10 + (ch - '0');
+            else { block += v; v = 0; }
+        }
+        hbh_batches::File& F = B->files[o.tid / B->batch_size];
+        std::string& s = F.pending;
+        s += R->id[o.qid]; s += '\t'; s += std::to_string(o.qlen); s += '\t'; s += std::to_string(o.qstart); s += '\t';
+        s += std::to_string(o.qend); s += '\t'; s += o.strand ? '-' : '+'; s += '\t'; s += R->id[o.tid]; s += '\t';
+        s += std::to_string(o.tlen); s += '\t'; s += std::to_string(o.tstart); s += '\t'; s += std::to_string(o.tend); s += '\t';
+        s += std::to_string(matches[i]); s += '\t'; s += std::to_string(block); s += '\t'; s.append((const char*)paf->buf.data() + paf->mapq[i].first, paf->mapq[i].second);
+        s += "\tcg:Z:"; s.append((const char*)o.cigar, o.cigar_len); s += '\n';
+        F.lines++;
+        B->written++;
+        if (s.size() >= (4u << 20) && !flush_batch(B, F, false)) return HB_ERR_INPUT;
+    }
+    return HB_OK;
+}
+
+// Finishes every file (frame end), frees `B`; lines_per_batch (may be NULL) receives each file's line count.
+int hbh_batches_close(hbh_batches* B, uint64_t* lines_per_batch) {
+    if (!B) return HB_ERR_ARG;
+    int rc = HB_OK;
+    for (size_t k = 0; k < B->files.size(); k++) {
+        hbh_batches::File& F = B->files[k];
+        if (F.f && F.cctx && rc == HB_OK && !flush_batch(B, F, true)) rc = HB_ERR_INPUT;  // ZSTD_e_end: the frame is complete
+        if (F.cctx) zstd().freeCCtx(F.cctx);
+        if (F.f && fclose(F.f) != 0 && rc == HB_OK) { t_err = "close failed"; rc = HB_ERR_INPUT; }
+        if (lines_per_batch) lines_per_batch[k] = F.lines;
+    }
+    delete B;
+    return rc;
+}
+
+// `herro align`: the FASTQ's reads (those of at least min_len bases) on device `device` in a context without weights, the PAF
+// streamed through hb_align_overlaps chunk_lines lines at a time, the aligned lines written as hbh_batches_write writes them.
+// times6: FASTQ load, context + upload, PAF read, alignment calls (wall), formatting + writing, total (s); counts7: lines read,
+// skipped (unknown names, self overlaps), aligned and written, of those at the band's edge, failed (not written), cells, device ms.
+int hbh_align(const char* reads_path, const char* paf_path, const char* out_dir, int device, uint32_t min_len, uint32_t band_w,
+              uint32_t batch_size, uint32_t chunk_lines, int io_threads, double* times6, uint64_t* counts7) {
+    if (!reads_path || !paf_path || !out_dir || !times6 || !counts7 || !chunk_lines) { t_err = "bad arguments"; return HB_ERR_ARG; }
+    const double t_begin = now_s();
+    std::fill(times6, times6 + 6, 0.0);
+    std::fill(counts7, counts7 + 7, 0ull);
+    hbh_reads* R = nullptr;
+    int rc = hbh_reads_load(reads_path, min_len, nullptr, 0, nullptr, 0, io_threads, &R);
+    if (rc) return rc;
+    times6[0] = now_s() - t_begin;
+    hb_ctx* ctx = nullptr;
+    hbh_paf* P = nullptr;
+    hbh_batches* B = nullptr;
+    double ms_dev = 0;
+    auto done = [&](int code) {
+        if (code && ctx && t_err.empty()) t_err = hb_last_error(ctx);
+        if (B) { const int c = hbh_batches_close(B, nullptr); if (!code) code = c; }
+        if (P) hbh_paf_close(P);
+        if (ctx) hb_destroy(ctx);
+        hbh_reads_free(R);
+        times6[5] = now_s() - t_begin;
+        counts7[6] = (uint64_t)ms_dev;
+        return code;
+    };
+    double t0 = now_s();
+    hb_options opt{};
+    opt.struct_size = sizeof opt; opt.window_size = std::max<uint32_t>(min_len, 1); opt.batch_size = 64; opt.flags = HB_FLAG_NO_MODEL;
+    if (hb_create(&ctx, device, nullptr, &opt) != HB_OK) { t_err = std::string("hb_create: ") + hb_last_error(nullptr); ctx = nullptr; return done(HB_ERR_CUDA); }
+    if (hb_upload_reads(ctx, hbh_reads_count(R), hbh_reads_word_ptrs(R), hbh_reads_lens(R), hbh_reads_qual_ptrs(R)) != HB_OK) {
+        t_err = std::string("hb_upload_reads: ") + hb_last_error(ctx);
+        return done(HB_ERR_CUDA);
+    }
+    times6[1] = now_s() - t0;
+    if ((rc = hbh_paf_open(paf_path, R, &P))) return done(rc);
+    if ((rc = hbh_batches_open(out_dir, R, batch_size, &B))) return done(rc);
+    std::vector<hb_overlap> out;
+    std::vector<uint8_t> text;
+    std::vector<int32_t> status;
+    std::vector<uint32_t> matches;
+    for (;;) {
+        t0 = now_s();
+        uint32_t n = 0;
+        if ((rc = hbh_paf_next(P, chunk_lines, &n))) return done(rc);
+        times6[2] += now_s() - t0;
+        if (!n) break;
+        t0 = now_s();
+        hb_align_shape sh{};
+        if ((rc = hb_align_overlaps(ctx, n, hbh_paf_overlaps(P), band_w, &sh))) { t_err = std::string("hb_align_overlaps: ") + hb_last_error(ctx); return done(rc); }
+        out.resize(n); text.resize(std::max<uint64_t>(sh.cigar_bytes, 1)); status.resize(n); matches.resize(n);
+        if ((rc = hb_align_fetch(ctx, &sh, out.data(), text.data(), status.data(), matches.data()))) { t_err = hb_last_error(ctx); return done(rc); }
+        times6[3] += now_s() - t0;
+        ms_dev += sh.ms_device;
+        counts7[4] += sh.n_failed;
+        counts7[3] += sh.n_band_edge;
+        counts7[2] += n - sh.n_failed;
+        counts7[5] += sh.cells;
+        t0 = now_s();
+        if ((rc = hbh_batches_write(B, P, out.data(), status.data(), matches.data(), n))) return done(rc);
+        times6[4] += now_s() - t0;
+    }
+    uint64_t c3[3];
+    hbh_paf_stats(P, c3);
+    counts7[0] = c3[0];
+    counts7[1] = c3[1];
+    t0 = now_s();
+    rc = hbh_batches_close(B, nullptr);
+    B = nullptr;
+    times6[4] += now_s() - t0;
+    return done(rc);
+}
+
+}  // extern "C"

@@ -59,6 +59,18 @@ def _lib():
                                 C.c_int, C.c_uint64, C.c_uint64, vp, vp]
     H.hbh_reads_store_bytes.argtypes = [vp]
     H.hbh_reads_store_bytes.restype = C.c_uint64
+    H.hbh_paf_open.argtypes = [C.c_char_p, vp, C.POINTER(vp)]
+    H.hbh_paf_next.argtypes = [vp, u32, C.POINTER(u32)]
+    H.hbh_paf_overlaps.argtypes = [vp]
+    H.hbh_paf_overlaps.restype = vp
+    H.hbh_paf_stats.argtypes = [vp, vp]
+    H.hbh_paf_stats.restype = None
+    H.hbh_paf_close.argtypes = [vp]
+    H.hbh_paf_close.restype = None
+    H.hbh_batches_open.argtypes = [C.c_char_p, vp, u32, C.POINTER(vp)]
+    H.hbh_batches_write.argtypes = [vp, vp, vp, vp, vp, u32]
+    H.hbh_batches_close.argtypes = [vp, vp]
+    H.hbh_align.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, u32, u32, u32, u32, C.c_int, vp, vp]
     H._io_ready = True
     return H
 
@@ -473,3 +485,89 @@ def inference(reads_path: str, alns_dir: str, model: str, output: str, window: i
                 fasta_close_s=t9[5], total_s=t9[6], corrected_bases=int(t9[7]), first_submit_s=t9[8], reads=int(c6[0]),
                 targets=int(c6[1]), records=int(c6[2]), failed_targets=int(c6[3]), alignment_peak_bytes=int(c6[4]),
                 alignment_budget_bytes=int(c6[5]))
+
+
+class PafReader:
+    """An overlap-only PAF (plain or gzip) in chunks of admitted lines (hbh_paf_*): unknown read names and self overlaps are skipped,
+    a cg:Z: field is ignored, repeated pairs are kept."""
+
+    def __init__(self, path: str, reads: Reads):
+        H = _lib()
+        self._H, self._h, self.reads = H, C.c_void_p(), reads
+        rc = H.hbh_paf_open(path.encode(), reads._h, C.byref(self._h))
+        if rc != 0:
+            raise api.HerroError(rc, H.hbh_last_error().decode())
+
+    def next(self, max_lines: int = 200_000):
+        """-> the next chunk's overlaps (OVERLAP_DTYPE, no CIGARs), or None at the end of the file.  The chunk stays current for
+        BatchWriter.write until the next call."""
+        n = C.c_uint32()
+        rc = self._H.hbh_paf_next(self._h, max_lines, C.byref(n))
+        if rc != 0:
+            raise api.HerroError(rc, self._H.hbh_last_error().decode())
+        if not n.value:
+            return None
+        buf = (C.c_char * (n.value * api.OVERLAP_DTYPE.itemsize)).from_address(self._H.hbh_paf_overlaps(self._h))
+        return np.frombuffer(buf, dtype=api.OVERLAP_DTYPE, count=n.value).copy()
+
+    def stats(self) -> dict:
+        c = np.zeros(3, np.uint64)
+        self._H.hbh_paf_stats(self._h, c.ctypes.data)
+        return dict(lines=int(c[0]), skipped=int(c[1]), bytes=int(c[2]))
+
+    def close(self):
+        if self._h:
+            self._H.hbh_paf_close(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class BatchWriter:
+    """`--read-alns` batches as the reference's write mode makes them (hbh_batches_*): <k>.oec.zst holds the k-th run of batch_size
+    reads in FASTQ order, a header (the count, then the ids) and the aligned lines of its targets in input order."""
+
+    def __init__(self, out_dir: str, reads: Reads, batch_size: int = 50_000):
+        H = _lib()
+        self._H, self._h, self.n_batches = H, C.c_void_p(), (reads.n + batch_size - 1) // batch_size
+        rc = H.hbh_batches_open(out_dir.encode(), reads._h, batch_size, C.byref(self._h))
+        if rc != 0:
+            raise api.HerroError(rc, H.hbh_last_error().decode())
+
+    def write(self, paf: PafReader, aligned: np.ndarray, status: np.ndarray, matches: np.ndarray):
+        """The current chunk of `paf` with the coordinates and CIGARs of `aligned` (Context.align's overlaps); lines whose status is
+        negative are not written."""
+        status = np.ascontiguousarray(status, np.int32)
+        matches = np.ascontiguousarray(matches, np.uint32)
+        aligned = np.ascontiguousarray(aligned)
+        rc = self._H.hbh_batches_write(self._h, paf._h, aligned.ctypes.data, status.ctypes.data, matches.ctypes.data, len(aligned))
+        if rc != 0:
+            raise api.HerroError(rc, self._H.hbh_last_error().decode())
+
+    def close(self) -> list:
+        """Finishes the files -> lines written per batch."""
+        lines = np.zeros(max(self.n_batches, 1), np.uint64)
+        h, self._h = self._h, C.c_void_p()
+        rc = self._H.hbh_batches_close(h, lines.ctypes.data)
+        if rc != 0:
+            raise api.HerroError(rc, self._H.hbh_last_error().decode())
+        return [int(x) for x in lines[:self.n_batches]]
+
+
+def align(reads_path: str, paf_path: str, out_dir: str, device: int = 0, min_len: int = 4096, band_w: int = 0, batch_size: int = 50_000,
+          chunk_lines: int = 200_000, io_threads: int = 0) -> dict:
+    """`herro align`, natively (hbh_align): an overlap-only PAF aligned on the device and written as `--read-alns` batches -> the
+    wall time of each phase and the counts."""
+    H = _lib()
+    t6, c7 = np.zeros(6), np.zeros(7, np.uint64)
+    rc = H.hbh_align(reads_path.encode(), paf_path.encode(), out_dir.encode(), device, min_len, band_w, batch_size, chunk_lines,
+                     io_threads or min(os.cpu_count() or 1, 32), t6.ctypes.data, c7.ctypes.data)
+    if rc != 0:
+        raise api.HerroError(rc, H.hbh_last_error().decode())
+    return dict(fastq_load_s=t6[0], upload_s=t6[1], paf_read_s=t6[2], align_s=t6[3], write_s=t6[4], total_s=t6[5], lines=int(c7[0]),
+                skipped=int(c7[1]), aligned=int(c7[2]), band_edge=int(c7[3]), failed=int(c7[4]), cells=int(c7[5]),
+                device_ms=int(c7[6]))

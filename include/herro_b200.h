@@ -235,6 +235,52 @@ int hb_features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, con
                       hb_features_shape* shape);
 int hb_features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_features_out* out, uint32_t flags, void* stream);
 
+/* ---- the base-level alignment of overlaps ------------------------------------------------- */
+#define HB_ALN_BAND_EDGE 1  /* hb_align_fetch status: aligned, but the path touched the band's edge (it may have left the band) */
+
+typedef struct hb_align_shape {     /* what one hb_align_overlaps produced                                                    */
+    uint64_t ticket;                /* names the result for hb_align_fetch                                                   */
+    uint32_t n_overlaps, n_failed, n_band_edge;
+    uint64_t cigar_bytes, cells;    /* total CIGAR text; DP cells computed, sum over aligned overlaps of (n + 1) * 2w         */
+    double ms_device;               /* device time of the alignment kernels                                                  */
+} hb_align_shape;
+
+/* The alignment `minimap2 -c` adds to an overlap-only PAF line, done on the device: per overlap (its cigar is ignored and may be
+ * NULL), a banded two-piece affine alignment of the target slice t[tstart, tend) against the query slice q[qstart, qend),
+ * reverse-complemented on strand 1, with minimap2's default scores (match 2, mismatch 4, gap min(4 + 2l, 24 + l)).  Row i of
+ * the n + 1 target rows holds the 2w columns c(i) - w <= j < c(i) + w (c(i) = floor(i m / n)) that lie in 0..m.  The traceback
+ * from (n, m) goes through the reference's fix_cigar (src/aligners.rs:138-250: indels flanked by matches left-aligned, a leading
+ * gap dropped, equal ops merged), then gaps left at either end are dropped too: the coordinates move inwards by the dropped
+ * lengths and the CIGAR, which starts and ends with M, spans them exactly.  DESIGN.md §12 gives the definition in full.
+ * hb_align_overlaps computes and fills *shape; hb_align_fetch copies out any subset of the results, as often as wanted:
+ *   out         [n] the input overlaps in input order with the new coordinates; cigar points into cigar_text (cigar_len bytes),
+ *               ready for hb_submit_alignments or hb_features_batch.  A failed overlap keeps its coordinates and has no CIGAR.
+ *   cigar_text  [shape->cigar_bytes] every CIGAR, back to back
+ *   status      [n] HB_OK, HB_ALN_BAND_EDGE, HB_ERR_INPUT (a coordinate outside its read, an empty span, or one span more than
+ *               twice the other) or HB_ERR_CAPACITY (its traceback alone exceeds the 8 GiB wave region)
+ *   matches     [n] identical base pairs inside M (PAF column 10); column 11 is the sum of the CIGAR's op lengths
+ * band_w: w, a multiple of 16 up to 256; 0 takes the default, 128.  Failed overlaps fail alone (the call returns HB_OK and
+ * hb_last_error names the first).
+ *
+ * Errors of the call (the previous result is gone):
+ *   HB_ERR_ARG       a NULL pointer, a qid or tid out of range, a strand other than 0 / 1, or a bad band_w
+ *   HB_ERR_STATE     no reads yet (hb_upload_reads / hb_attach_read_store); for fetch, a shape whose ticket is not the latest result
+ *   HB_ERR_CUDA      a CUDA failure
+ *
+ * Synchronous: both calls return when their work is done.  The overlaps run in waves whose traceback (one byte per cell) and
+ * op slots fit a grow-only region, longest overlaps first.  A wave takes at most 8 GiB and at most half of the device memory
+ * that is free when the call starts (the region's own bytes count as free); the region stays allocated until the context is
+ * destroyed.  With a host read store the call's reads are
+ * gathered once, as a launch gathers its own.  Works on an HB_FLAG_NO_MODEL context.
+ *
+ * Threading: calls of hb_align_overlaps / hb_align_fetch on one context serialise among themselves on a lane of their own; they may
+ * run beside hb_submit_*, hb_flush, hb_poll_corrected and the other single-stage calls (not beside hb_upload_reads).
+ *
+ * Counters: adds to kernel_launches, h2d_bytes, d2h_bytes and host_allocs when scratch grows; the kernel time and the cells are in
+ * the shape. */
+int hb_align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band_w, hb_align_shape* shape);
+int hb_align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8_t* cigar_text, int32_t* status, uint32_t* matches);
+
 /* ---- the model call alone ---------------------------------------------------------------- */
 #define HB_FWD_DEVICE_PTRS 1u  /* bases, quals and both outputs are device pointers on the context's device */
 /* The replacement of inference() (src/inference.rs:147-175) on one collated batch, for a host that keeps its own features stage,
