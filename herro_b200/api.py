@@ -64,6 +64,18 @@ class HbAlignShape(C.Structure):
                [(n, C.c_uint64) for n in ("cigar_bytes", "cells")] + [("ms_device", C.c_double)]
 
 
+OVL_PARAM_NAMES = ("k", "w", "min_score", "min_anchors", "max_gap", "bandwidth", "max_iter", "top_frac_ppm", "min_occ")
+
+
+class HbOvlParams(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in OVL_PARAM_NAMES]
+
+
+class HbOvlShape(C.Structure):
+    _fields_ = [("ticket", C.c_uint64)] + [(n, C.c_uint32) for n in ("n_targets", "n_overlaps", "max_occ", "n_filtered_hashes")] + \
+               [(n, C.c_uint64) for n in ("index_entries", "query_minimizers", "anchors", "chained_groups")] + [("ms_device", C.c_double)]
+
+
 FEATURES_OUT_FIELDS = ("status", "n_windows", "rows", "n_alns", "n_sup", "n_ids", "bases", "quals", "supported", "indices", "ids",
                        "batch_B", "batch_Lmax", "batch_win", "batch_bases", "batch_quals")
 
@@ -131,6 +143,8 @@ def load_library():
     L.hb_features_fetch.argtypes = [vp, C.POINTER(HbFeaturesShape), C.POINTER(HbFeaturesOut), u32, vp]
     L.hb_align_overlaps.argtypes = [vp, u32, vp, u32, C.POINTER(HbAlignShape)]
     L.hb_align_fetch.argtypes = [vp, C.POINTER(HbAlignShape), vp, vp, vp, vp]
+    L.hb_find_overlaps.argtypes = [vp, u32, vp, C.POINTER(HbOvlParams), C.POINTER(HbOvlShape)]
+    L.hb_find_fetch.argtypes = [vp, C.POINTER(HbOvlShape), vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -140,7 +154,7 @@ EXPORTED_SYMBOLS = ["hb_inspect_model", "hb_dump_features", "hb_window_range", "
                     "hb_debug_window_shape", "hb_debug_dump_window", "hb_replay_last_launch", "hb_selftest_gemm",
                     "hb_inspect_model_ex", "hb_selftest_pos_attention", "hb_forward_batch", "hb_consensus_batch",
                     "hb_features_batch", "hb_features_fetch", "hb_read_store_create", "hb_read_store_destroy", "hb_attach_read_store",
-                    "hb_align_overlaps", "hb_align_fetch"]
+                    "hb_align_overlaps", "hb_align_fetch", "hb_find_overlaps", "hb_find_fetch"]
 HB_FWD_DEVICE_PTRS = 1
 HB_CONS_DEVICE_PTRS = 1
 HB_FEAT_DEVICE_PTRS = 1
@@ -684,6 +698,27 @@ class Context:
         cigars = [text[int(o["cigar"]) - base:int(o["cigar"]) - base + int(o["cigar_len"])].tobytes() if o["cigar"] else b"" for o in out]
         shape = {f: getattr(sh, f) for f, _ in HbAlignShape._fields_}
         return dict(overlaps=out, cigar_text=text, cigars=cigars, status=status, matches=matches, shape=shape)
+
+    # -- all-vs-all overlaps ---------------------------------------------------------------
+    def find_overlaps(self, target_rids, **params) -> dict:
+        """The overlaps of every read in the store against the reads target_rids (hb_find_overlaps + hb_find_fetch); params are
+        hb_ovl_params fields (k, w, min_score, min_anchors, max_gap, bandwidth, max_iter, top_frac_ppm, min_occ), 0 or absent
+        for the default.  -> dict(overlaps: OVERLAP_DTYPE without CIGARs, in target order then ascending qid, score, n_anchors,
+        covered: u32 each, shape: dict of hb_ovl_shape)"""
+        unknown = set(params) - set(OVL_PARAM_NAMES)
+        if unknown:
+            raise TypeError(f"unknown overlap parameters: {sorted(unknown)}")
+        tg = np.ascontiguousarray(target_rids, np.uint32)
+        p = HbOvlParams(*(int(params.get(n) or 0) for n in OVL_PARAM_NAMES))
+        sh = HbOvlShape()
+        self._check(self._L.hb_find_overlaps(self._h, len(tg), tg.ctypes.data if len(tg) else None, C.byref(p), C.byref(sh)))
+        n = sh.n_overlaps
+        out = np.zeros(max(n, 1), OVERLAP_DTYPE)
+        score, n_anchors, covered = (np.zeros(max(n, 1), np.uint32) for _ in range(3))
+        self._check(self._L.hb_find_fetch(self._h, C.byref(sh), out.ctypes.data, score.ctypes.data, n_anchors.ctypes.data,
+                                          covered.ctypes.data))
+        shape = {f: getattr(sh, f) for f, _ in HbOvlShape._fields_}
+        return dict(overlaps=out[:n], score=score[:n], n_anchors=n_anchors[:n], covered=covered[:n], shape=shape)
 
     def set_launch_targets(self, n: int):
         self._check(self._L.hb_set_launch_targets(self._h, n))

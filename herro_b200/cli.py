@@ -5,6 +5,11 @@ as a thin argument parser over the native host pipeline (herro_b200/host/io.cpp 
     python -m herro_b200.cli inference --torch --read-alns <dir> -d 0 -m model.pt -b 64 reads.fastq out.fasta
                                        (any TorchScript graph with the reference's forward signature, run by torch.jit)
     python -m herro_b200.cli features  --read-alns <dir> reads.fastq out_dir
+    python -m herro_b200.cli inference [--write-alns <dir>] -m model.hbw -b 64 reads.fastq out.fasta
+                                       (also `features`: without --read-alns the overlaps are found and aligned on the first
+                                       device of -d, as `overlap` then `align`, into --write-alns or a temporary directory)
+    python -m herro_b200.cli overlap -d 0 [-w 4096] [--targets-per-call 50000] [-k 25 -W 17 ...] reads.fastq out.paf[.gz]
+                                       (all-vs-all read overlaps found on the device, written as overlap-only PAF)
     python -m herro_b200.cli align -d 0 [-w 4096] [--band W] [--batch-size 50000] reads.fastq overlaps.paf[.gz] out_dir
                                        (the CIGARs of an overlap-only PAF aligned on the device, written as --read-alns batches)
     python -m herro_b200.cli predict   -m model.hbw -b 64 [-d 0] features_dir out_dir   (the model alone, on `features` output)
@@ -25,7 +30,9 @@ from __future__ import annotations
 
 import argparse
 import os
+import shutil
 import sys
+import tempfile
 
 from . import api, hostio
 
@@ -193,6 +200,38 @@ def consensus(args):
     print(f"Wrote {records} records ({bases} bases) to {args.output}.", file=sys.stderr)
 
 
+OVL_FLAGS = (("-k", "k"), ("-W", "w"), ("--min-score", "min_score"), ("--min-anchors", "min_anchors"), ("--max-gap", "max_gap"),
+             ("--bandwidth", "bandwidth"), ("--max-iter", "max_iter"), ("--top-frac-ppm", "top_frac_ppm"), ("--min-occ", "min_occ"))
+
+
+def overlap(args):
+    r = hostio.overlap(args.reads, args.output, device=args.device, min_len=args.window_size, targets_per_call=args.targets_per_call,
+                       **{p: getattr(args, p) for _, p in OVL_FLAGS})
+    print(f"Found {r['overlaps']} overlaps among {r['reads']} reads in {r['calls']} calls, {r['device_ms'] / 1e3:.2f} s on the device.  "
+          f"Wall time: FASTQ {r['fastq_load_s']:.2f} s, context and upload {r['upload_s']:.2f} s, overlap calls {r['find_s']:.2f} s, "
+          f"writing {r['write_s']:.2f} s, total {r['total_s']:.2f} s.", file=sys.stderr)
+    return r
+
+
+def generate_alignments(args):
+    """Without --read-alns: `overlap` into a PAF, then `align` into --write-alns DIR or a temporary directory, on the first device
+    of -d; args.read_alns then names that directory.  Returns the temporary directory to remove, or None."""
+    dev = int(str(getattr(args, "devices", 0)).split(",")[0])
+    tmp = tempfile.mkdtemp(prefix="herro_alns_")
+    out = args.write_alns or os.path.join(tmp, "alns")
+    paf = os.path.join(tmp, "overlaps.paf")
+    overlap(argparse.Namespace(reads=args.reads, output=paf, device=dev, window_size=args.window_size, targets_per_call=50_000,
+                               **{p: 0 for _, p in OVL_FLAGS}))
+    align(argparse.Namespace(reads=args.reads, paf=paf, output=out, device=dev, window_size=args.window_size, band=0,
+                             batch_size=50_000))
+    os.remove(paf)
+    args.read_alns = out
+    if args.write_alns:
+        shutil.rmtree(tmp)
+        return None
+    return tmp
+
+
 def align(args):
     r = hostio.align(args.reads, args.paf, args.output, device=args.device, min_len=args.window_size, band_w=args.band,
                      batch_size=args.batch_size)
@@ -208,7 +247,9 @@ def main(argv=None):
     ap = argparse.ArgumentParser(prog="herro_b200")
     sub = ap.add_subparsers(dest="cmd", required=True)
     inf = sub.add_parser("inference")
-    inf.add_argument("--read-alns", required=True, help="directory with *.oec.zst alignment batches")
+    src = inf.add_mutually_exclusive_group()
+    src.add_argument("--read-alns", help="directory with *.oec.zst alignment batches (absent: found and aligned on the device)")
+    src.add_argument("--write-alns", help="find and align the overlaps on the device and keep the batches in this directory")
     inf.add_argument("-w", dest="window_size", type=int, default=4096)
     inf.add_argument("-t", dest="feat_gen_threads", type=int, default=1)
     inf.add_argument("-m", dest="model", required=True)
@@ -222,12 +263,22 @@ def main(argv=None):
     inf.add_argument("reads")
     inf.add_argument("output")
     ft = sub.add_parser("features")
-    ft.add_argument("--read-alns", required=True)
+    src = ft.add_mutually_exclusive_group()
+    src.add_argument("--read-alns", help="directory with *.oec.zst alignment batches (absent: found and aligned on the device)")
+    src.add_argument("--write-alns", help="find and align the overlaps on the device and keep the batches in this directory")
     ft.add_argument("-w", dest="window_size", type=int, default=4096)
     ft.add_argument("-m", dest="model", default=None, help="accepted and ignored: the feature files do not depend on the model")
     ft.add_argument("--targets-per-launch", type=int, default=256, help="targets per features call")
     ft.add_argument("reads")
     ft.add_argument("output")
+    ov = sub.add_parser("overlap", help="all-vs-all read overlaps found on the device, written as overlap-only PAF")
+    ov.add_argument("-d", dest="device", type=int, default=0)
+    ov.add_argument("-w", dest="window_size", type=int, default=4096, help="reads shorter than this are not loaded, as in inference")
+    ov.add_argument("--targets-per-call", type=int, default=50_000, help="target reads per hb_find_overlaps call")
+    for flag, p in OVL_FLAGS:
+        ov.add_argument(flag, dest=p, type=int, default=0, help=f"hb_ovl_params.{p} (0: the default)")
+    ov.add_argument("reads")
+    ov.add_argument("output")
     al = sub.add_parser("align", help="the CIGARs of an overlap-only PAF (minimap2 without -c), written as --read-alns batches")
     al.add_argument("-d", dest="device", type=int, default=0)
     al.add_argument("-w", dest="window_size", type=int, default=4096, help="reads shorter than this are not loaded, as in inference")
@@ -251,19 +302,24 @@ def main(argv=None):
     cs.add_argument("reads")
     cs.add_argument("output")
     args = ap.parse_args(argv)
-    if args.cmd == "inference":
-        if args.torch:
-            if args.cluster:
-                raise SystemExit("-c is not supported with --torch")
-            return inference_torch(args)
-        return inference(args)
+    if args.cmd in ("inference", "features"):
+        if args.cmd == "inference" and args.torch and args.cluster:
+            raise SystemExit("-c is not supported with --torch")
+        tmp = generate_alignments(args) if not args.read_alns else None
+        try:
+            if args.cmd == "features":
+                return features(args)
+            return inference_torch(args) if args.torch else inference(args)
+        finally:
+            if tmp:
+                shutil.rmtree(tmp, ignore_errors=True)
+    if args.cmd == "overlap":
+        return overlap(args)
     if args.cmd == "align":
         return align(args)
     if args.cmd == "predict":
         return predict(args)
-    if args.cmd == "consensus":
-        return consensus(args)
-    return features(args)
+    return consensus(args)
 
 
 if __name__ == "__main__":

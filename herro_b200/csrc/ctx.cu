@@ -257,6 +257,14 @@ struct AlnResult {
     std::vector<uint8_t> text;
 };
 
+// What one hb_find_overlaps produced, in call-target order then ascending qid, until hb_find_fetch copies it out
+struct OvlResult {
+    bool valid = false;
+    hb_ovl_shape shape{};
+    std::vector<hb_overlap> ovl;
+    std::vector<uint32_t> score, n_anchors, covered;
+};
+
 }  // namespace
 
 // The read store in host memory (hb_read_store_create): every read's words and qualities in one page-locked block that every
@@ -369,6 +377,20 @@ struct hb_ctx {
         uint64_t wave_bytes = 8ull << 30;  // traceback bytes and op slots of one wave; HERRO_B200_ALN_WAVE_BYTES: tests shrink it to
                                            // run several waves
     } aln;
+    // hb_find_overlaps' lane: a LaneBase; the gathered reads of the targets and of a query chunk (host store); the index (entries,
+    // distinct hashes, table); a chunk's minimizers, anchors and groups; CUB's scratch; all grow-only.  Calls of hb_find_overlaps
+    // and hb_find_fetch serialise on its mutex.
+    struct OvlLane : LaneBase {
+        std::mutex mu;
+        DevBuf d_treads, d_qreads, d_lists, d_ent, d_tab, d_hash, d_qmin, d_anc, d_grp, d_tmp;
+        PinBuf pin;  // small copies out: counts, the chosen quantile, the kept groups
+        PinVec<ReadCopy> read_list;
+        std::vector<uint32_t> stamp;
+        uint32_t stamp_gen = 0;
+        OvlResult res;
+        uint64_t ticket = 0;
+        uint64_t chunk_bases = ~0ull;  // query bases per chunk at most; HERRO_B200_OVL_CHUNK_BASES: tests shrink it to run many chunks
+    } ovl;
     bool no_model = false;  // HB_FLAG_NO_MODEL: no weights; the calls that run the forward refuse
 
     std::deque<Result> results;
@@ -2408,6 +2430,346 @@ int align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8
     return HB_OK;
 }
 
+// ---------------------------------------------------------------------------------- hb_find_overlaps / hb_find_fetch
+constexpr uint32_t OVL_DEFAULTS[9] = {25, 17, 2500, 3, 5000, 150, 5000, 5000, 10};
+constexpr uint64_t OVL_ANCHOR_BYTES = 56;  // per anchor of a chunk: two (group, position) buffers, f, pred, and a group's slot
+
+// Runs the CUB primitive `f(tmp, bytes)` with its scratch in `tmp`
+template <class F>
+cudaError_t cub_call(DevBuf& tmp, F f) {
+    size_t bytes = 0;
+    cudaError_t e = f(nullptr, bytes);
+    if (e == cudaSuccess) e = tmp.grow(std::max<size_t>(bytes, 1));
+    if (e == cudaSuccess) e = f(tmp.p, bytes);
+    return e;
+}
+
+// The reads `rids[0..n)` as a store view: the uploaded store, or with a host store the reads gathered into `region`
+int ovl_gather(hb_ctx* ctx, hb_ctx::OvlLane& O, DevBuf& region, const uint32_t* rids, size_t n, ReadStoreView& rs, hb_stats& S) {
+    rs = ctx->rs;
+    if (!ctx->store) return HB_OK;
+    GatherSizes gs;
+    ReadsInArgs g{};
+    const int rc = list_reads(ctx, O.read_list, O.stamp, O.stamp_gen, n, [&](auto& add) {
+        for (size_t i = 0; i < n; i++) add(rids[i]);
+    }, gs);
+    if (rc) return rc;
+    g.src_words = ctx->store_words;
+    g.src_qual = ctx->store_qual;
+    Carve c{nullptr};
+    carve_gather(c, gs, g, rs);
+    CK(region.grow(c.bytes));
+    Carve c2{region.as<uint8_t>()};
+    carve_gather(c2, gs, g, rs);
+    CK(cudaMemcpyAsync((void*)g.list, O.read_list.data(), vbytes(O.read_list), cudaMemcpyHostToDevice, O.stream));
+    KTimer kt;  // the gather's time is part of the call's, not of a kernel class of hb_stats
+    S.kernel_launches += launch_reads_in(g, O.stream, kt);
+    S.h2d_bytes += vbytes(O.read_list) + gs.words * 8 + gs.qual;
+    return HB_OK;
+}
+
+struct OvlRec {
+    uint32_t tpos;
+    hb_overlap o;
+    uint32_t score, n_anchors, covered;
+};
+
+// The work of hb_find_overlaps, with the lane's lock held and the context's device current
+int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl_params* params, hb_ovl_shape* shape) {
+    hb_ctx::OvlLane& O = ctx->ovl;
+    OvlResult& R = O.res;
+    R.valid = false;
+    if (!shape || !trids) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (!n_t) return fail(ctx, HB_ERR_ARG, "n_targets must be positive");
+    uint32_t pv[9];
+    static_assert(sizeof(hb_ovl_params) == sizeof pv, "hb_ovl_params is nine uint32_t");
+    if (params) memcpy(pv, params, sizeof pv); else memset(pv, 0, sizeof pv);
+    for (int i = 0; i < 9; i++) if (!pv[i]) pv[i] = OVL_DEFAULTS[i];
+    const uint32_t k = pv[0], w = pv[1], min_score = pv[2], min_anchors = pv[3], max_gap = pv[4], bandwidth = pv[5],
+                   max_iter = pv[6], top_frac_ppm = pv[7], min_occ = pv[8];
+    if (k < 12 || k > 28) return fail(ctx, HB_ERR_ARG, "k must be 12..28");
+    if (w < 2 || w > 32) return fail(ctx, HB_ERR_ARG, "w must be 2..32");
+    if (top_frac_ppm >= 1000000) return fail(ctx, HB_ERR_ARG, "top_frac_ppm must be below 1000000");
+    if (min_score > (1u << 30) || max_gap > (1u << 30) || bandwidth > (1u << 30) || max_iter > (1u << 30))
+        return fail(ctx, HB_ERR_ARG, "min_score, max_gap, bandwidth and max_iter must be at most 2^30");
+    if (!ctx->have_reads) return fail(ctx, HB_ERR_STATE, "hb_upload_reads or hb_attach_read_store must be called before hb_find_overlaps");
+    const uint32_t n_reads = ctx->n_reads;
+    {
+        std::vector<uint8_t> seen(n_reads, 0);
+        for (uint32_t i = 0; i < n_t; i++) {
+            if (trids[i] >= n_reads) return fail(ctx, HB_ERR_INPUT, "target " + std::to_string(i) + ": read id out of range");
+            if (seen[trids[i]]++) return fail(ctx, HB_ERR_INPUT, "target " + std::to_string(i) + ": read id repeated");
+        }
+    }
+    const cudaStream_t st = O.stream;
+    hb_stats S{};
+    hb_ovl_shape sh{};
+    double ms_dev = 0;
+    size_t mem_free = 0, mem_total = 0;
+    CK(cudaMemGetInfo(&mem_free, &mem_total));
+    const uint64_t budget = O.d_anc.cap + mem_free / 2;
+    auto timed_sync = [&]() -> int {
+        CK(cudaEventRecord(O.ev[2], st));
+        CK(cudaStreamSynchronize(st));
+        float ms = 0;
+        CK(cudaEventElapsedTime(&ms, O.ev[1], O.ev[2]));
+        ms_dev += ms;
+        CK(cudaEventRecord(O.ev[1], st));
+        return HB_OK;
+    };
+    // ---- lists: the targets and every read (the queries), counts and counters
+    std::vector<uint32_t> h_rids(n_reads), h_tlen(n_t);
+    for (uint32_t r = 0; r < n_reads; r++) h_rids[r] = r;
+    for (uint32_t i = 0; i < n_t; i++) h_tlen[i] = ctx->read_len[trids[i]];
+    uint32_t *d_trids, *d_tlens, *d_rids, *d_lens, *d_ctr;
+    uint64_t *d_tcnt, *d_qcnt;
+    auto carve_lists = [&](Carve& c) {
+        c(d_trids, n_t); c(d_tlens, n_t); c(d_rids, n_reads); c(d_lens, n_reads); c(d_ctr, 8);
+        c(d_tcnt, (size_t)n_t + 1); c(d_qcnt, (size_t)n_reads + 1);
+    };
+    {
+        Carve c{nullptr};
+        carve_lists(c);
+        CK(O.d_lists.grow(c.bytes));
+        Carve c2{O.d_lists.as<uint8_t>()};
+        carve_lists(c2);
+    }
+    CK(O.pin.grow(256));
+    uint64_t* pin64 = O.pin.as<uint64_t>();
+    uint32_t* pin32 = O.pin.as<uint32_t>();
+    CK(cudaEventRecord(O.ev[1], st));
+    CK(cudaMemcpyAsync(d_trids, trids, n_t * 4ull, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tlens, h_tlen.data(), n_t * 4ull, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_rids, h_rids.data(), n_reads * 4ull, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_lens, ctx->read_len.data(), n_reads * 4ull, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_ctr, 0, 32, st));
+    S.h2d_bytes += 8ull * (n_t + n_reads);
+    // ---- the index: the targets' minimizers sorted by hash, the occurrence threshold, the table
+    ReadStoreView trs;
+    int rc = ovl_gather(ctx, O, O.d_treads, trids, n_t, trs, S);
+    if (rc) return rc;
+    OvlSketchArgs sk{trs, d_trids, d_tlens, n_t, k, w, d_tcnt, d_tcnt, nullptr, nullptr};
+    CK(cudaMemsetAsync(d_tcnt, 0, 8ull * (n_t + 1), st));
+    launch_ovl_sketch(sk, false, st);
+    CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_exclusive_sum(t, b, d_tcnt, (uint64_t)n_t + 1, st); }));
+    CK(cudaMemcpyAsync(pin64, d_tcnt + n_t, 8, cudaMemcpyDeviceToHost, st));
+    if ((rc = timed_sync())) return rc;
+    const uint64_t E = pin64[0];
+    if (E >= (1ull << 32)) return fail(ctx, HB_ERR_CAPACITY, "the index holds 2^32 minimizers or more");
+    uint64_t *ek[2], *ev[2];
+    {
+        auto carve = [&](Carve& c) { c(ek[0], E); c(ek[1], E); c(ev[0], E); c(ev[1], E); };
+        Carve c{nullptr};
+        carve(c);
+        CK(O.d_ent.grow(std::max<size_t>(c.bytes, 256)));
+        Carve c2{O.d_ent.as<uint8_t>()};
+        carve(c2);
+    }
+    sk.key = ek[0];
+    sk.val = ev[0];
+    launch_ovl_sketch(sk, true, st);
+    int esel = 0;
+    if (E) CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_sort_pairs(t, b, ek, ev, esel, E, 2 * k, st); }));
+    uint64_t* uniq;
+    uint32_t *occ, *occ_off, *occ_sorted;
+    {
+        auto carve = [&](Carve& c) { c(uniq, E); c(occ, E); c(occ_off, E); c(occ_sorted, E); };
+        Carve c{nullptr};
+        carve(c);
+        CK(O.d_tab.grow(std::max<size_t>(c.bytes, 256)));
+        Carve c2{O.d_tab.as<uint8_t>()};
+        carve(c2);
+    }
+    if (E) CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_runs(t, b, ek[esel], uniq, occ, d_ctr, E, st); }));
+    CK(cudaMemcpyAsync(pin32, d_ctr, 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = timed_sync())) return rc;
+    const uint32_t n_d = pin32[0];
+    uint32_t max_occ = min_occ;
+    if (n_d) {
+        CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_exclusive_sum_u32(t, b, occ, occ_off, n_d, st); }));
+        CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_sort_u32(t, b, occ, occ_sorted, n_d, st); }));
+        const uint64_t rank = std::min<uint64_t>((1000000ull - top_frac_ppm) * n_d / 1000000ull, n_d - 1);
+        CK(cudaMemcpyAsync(pin32, occ_sorted + rank, 4, cudaMemcpyDeviceToHost, st));
+        if ((rc = timed_sync())) return rc;
+        max_occ = std::max(min_occ, pin32[0]);
+    }
+    uint64_t tcap = 1024;
+    while (tcap < 2ull * n_d) tcap <<= 1;
+    OvlTableArgs ta{uniq, occ, occ_off, n_d, max_occ, nullptr, nullptr, tcap - 1, d_ctr + 1};
+    {
+        auto carve = [&](Carve& c) { c(ta.keys, tcap); c(ta.vals, tcap); };
+        Carve c{nullptr};
+        carve(c);
+        CK(O.d_hash.grow(c.bytes));
+        Carve c2{O.d_hash.as<uint8_t>()};
+        carve(c2);
+    }
+    CK(cudaMemsetAsync(ta.keys, 0xff, tcap * 8, st));
+    launch_ovl_table(ta, st);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(pin32, d_ctr + 1, 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = timed_sync())) return rc;
+    S.kernel_launches += 3 + 5;  // sketch x2, table; CUB: scan, sort, runs, scan, sort
+    sh.n_filtered_hashes = pin32[0];
+    sh.max_occ = max_occ;
+    sh.index_entries = E;
+    // ---- the queries, in chunks of reads in rid order: sketch, anchors, sort, groups, chains
+    std::vector<OvlRec> recs;
+    uint64_t chunk = O.chunk_bases;
+    int qbits = 1;
+    for (uint32_t q0 = 0; q0 < n_reads;) {
+        uint32_t q1 = q0 + 1;
+        uint64_t bases = ctx->read_len[q0];
+        while (q1 < n_reads && q1 - q0 < (1u << 30) && bases + ctx->read_len[q1] <= chunk) bases += ctx->read_len[q1++];
+        const uint32_t nq = q1 - q0;
+        CK(cudaEventRecord(O.ev[1], st));
+        ReadStoreView qrs;
+        if ((rc = ovl_gather(ctx, O, O.d_qreads, h_rids.data() + q0, nq, qrs, S))) return rc;
+        OvlSketchArgs qs{qrs, d_rids + q0, d_lens + q0, nq, k, w, d_qcnt, d_qcnt, nullptr, nullptr};
+        CK(cudaMemsetAsync(d_qcnt, 0, 8ull * (nq + 1), st));
+        launch_ovl_sketch(qs, false, st);
+        CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_exclusive_sum(t, b, d_qcnt, (uint64_t)nq + 1, st); }));
+        CK(cudaMemcpyAsync(pin64, d_qcnt + nq, 8, cudaMemcpyDeviceToHost, st));
+        if ((rc = timed_sync())) return rc;
+        const uint64_t M = pin64[0];
+        OvlAnchorArgs an{ta.keys, ta.vals, ta.mask, ev[esel], d_trids, nullptr, nullptr, M, d_rids + q0, d_lens + q0, k,
+                         nullptr, nullptr, nullptr, nullptr};
+        {
+            uint64_t *mk, *mv, *ac;
+            auto carve = [&](Carve& c) { c(mk, M); c(mv, M); c(ac, M + 1); };
+            Carve c{nullptr};
+            carve(c);
+            CK(O.d_qmin.grow(c.bytes));
+            Carve c2{O.d_qmin.as<uint8_t>()};
+            carve(c2);
+            qs.key = mk; qs.val = mv;
+            an.mkey = mk; an.mval = mv; an.count = ac; an.offset = ac;
+        }
+        launch_ovl_sketch(qs, true, st);
+        CK(cudaMemsetAsync(an.count, 0, 8 * (M + 1), st));
+        launch_ovl_anchors(an, false, st);
+        CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_exclusive_sum(t, b, an.count, M + 1, st); }));
+        CK(cudaMemcpyAsync(pin64, an.count + M, 8, cudaMemcpyDeviceToHost, st));
+        if ((rc = timed_sync())) return rc;
+        S.kernel_launches += 3 + 2;
+        const uint64_t A = pin64[0];
+        if (A * OVL_ANCHOR_BYTES > budget || A > (uint64_t)INT32_MAX) {
+            if (nq == 1) return fail(ctx, HB_ERR_CAPACITY, "read " + std::to_string(q0) + ": its anchors exceed the anchor region");
+            chunk = std::max<uint64_t>(bases / 2, 1);  // fewer reads per chunk from here on
+            continue;
+        }
+        uint64_t *ak[2], *axy[2], *guniq;
+        int32_t *f, *pred;
+        uint32_t* gcnt;
+        {
+            auto carve = [&](Carve& c) { c(ak[0], A); c(ak[1], A); c(axy[0], A); c(axy[1], A); c(f, A); c(pred, A); c(guniq, A); c(gcnt, A); };
+            Carve c{nullptr};
+            carve(c);
+            CK(O.d_anc.grow(std::max<size_t>(c.bytes, 256), false));
+            Carve c2{O.d_anc.as<uint8_t>()};
+            carve(c2);
+        }
+        an.gkey = ak[0];
+        an.xy = axy[0];
+        launch_ovl_anchors(an, true, st);
+        while ((1ull << qbits) < nq) qbits++;
+        int asel = 0;
+        CK(cudaMemsetAsync(d_ctr + 2, 0, 4, st));
+        if (A) {
+            CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_sort_pairs(t, b, axy, ak, asel, A, 64, st); }));
+            CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_sort_pairs(t, b, ak, axy, asel, A, 33 + qbits, st); }));
+            CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_runs(t, b, ak[asel], guniq, gcnt, d_ctr + 2, A, st); }));
+        }
+        CK(cudaMemcpyAsync(pin32, d_ctr + 2, 4, cudaMemcpyDeviceToHost, st));
+        if ((rc = timed_sync())) return rc;
+        const uint32_t G = pin32[0];
+        uint32_t* goff;
+        OvlGroup *gout, *gkept;
+        {
+            auto carve = [&](Carve& c) { c(goff, G); c(gout, G); c(gkept, G); };
+            Carve c{nullptr};
+            carve(c);
+            CK(O.d_grp.grow(std::max<size_t>(c.bytes, 256)));
+            Carve c2{O.d_grp.as<uint8_t>()};
+            carve(c2);
+        }
+        CK(cudaMemsetAsync(d_ctr + 3, 0, 8, st));
+        uint32_t n_kept = 0;
+        if (G) {
+            CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_exclusive_sum_u32(t, b, gcnt, goff, G, st); }));
+            OvlChainArgs ch{guniq, gcnt, goff, G, axy[asel], f, pred, k, min_score, min_anchors, max_gap, bandwidth, max_iter,
+                            gout, d_ctr + 3};
+            launch_ovl_chain(ch, st);
+            CK(cudaGetLastError());
+            CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_select_kept(t, b, gout, gkept, d_ctr + 4, G, st); }));
+        }
+        CK(cudaMemcpyAsync(pin32, d_ctr + 3, 8, cudaMemcpyDeviceToHost, st));
+        if ((rc = timed_sync())) return rc;
+        S.kernel_launches += 1 + 3 + (G ? 3 : 0);
+        sh.chained_groups += pin32[0];
+        n_kept = pin32[1];
+        if (n_kept) {
+            CK(O.pin.grow(std::max<size_t>(256, n_kept * sizeof(OvlGroup))));
+            pin64 = O.pin.as<uint64_t>();
+            pin32 = O.pin.as<uint32_t>();
+            CK(cudaMemcpyAsync(O.pin.p, gkept, n_kept * sizeof(OvlGroup), cudaMemcpyDeviceToHost, st));
+            if ((rc = timed_sync())) return rc;
+            S.d2h_bytes += n_kept * sizeof(OvlGroup);
+        }
+        S.d2h_bytes += 4 * 8;
+        sh.query_minimizers += M;
+        sh.anchors += A;
+        // ---- one record per (target, query): the better strand, strand 0 on ties
+        const OvlGroup* kg = O.pin.as<OvlGroup>();
+        for (uint32_t i = 0; i < n_kept; i++) {
+            const OvlGroup& g = kg[i];
+            if (i + 1 < n_kept && (kg[i + 1].gkey >> 1) == (g.gkey >> 1) && kg[i + 1].score > g.score) continue;
+            if (i > 0 && (kg[i - 1].gkey >> 1) == (g.gkey >> 1) && kg[i - 1].score >= g.score) continue;
+            const uint32_t qc = (uint32_t)(g.gkey >> 33), t = (uint32_t)(g.gkey >> 1), s = (uint32_t)(g.gkey & 1);
+            const uint32_t qid = q0 + qc, qlen = ctx->read_len[qid], tid = trids[t];
+            OvlRec r{t, hb_overlap{}, (uint32_t)g.score, g.n_anchors, g.covered};
+            r.o.qid = qid; r.o.qlen = qlen; r.o.strand = s;
+            r.o.tid = tid; r.o.tlen = ctx->read_len[tid];
+            r.o.tstart = g.x_first - k + 1; r.o.tend = g.x_last + 1;
+            if (s == 0) { r.o.qstart = g.y_first - k + 1; r.o.qend = g.y_last + 1; }
+            else { r.o.qstart = qlen - g.y_last - 1; r.o.qend = qlen - g.y_first + k - 1; }
+            recs.push_back(r);
+        }
+        q0 = q1;
+    }
+    std::stable_sort(recs.begin(), recs.end(), [](const OvlRec& a, const OvlRec& b) { return a.tpos < b.tpos; });
+    const size_t n = recs.size();
+    R.ovl.resize(n); R.score.resize(n); R.n_anchors.resize(n); R.covered.resize(n);
+    for (size_t i = 0; i < n; i++) {
+        R.ovl[i] = recs[i].o;
+        R.score[i] = recs[i].score; R.n_anchors[i] = recs[i].n_anchors; R.covered[i] = recs[i].covered;
+    }
+    sh.ticket = ++O.ticket;
+    sh.n_targets = n_t;
+    sh.n_overlaps = (uint32_t)n;
+    sh.ms_device = ms_dev;
+    R.shape = sh;
+    R.valid = true;
+    *shape = sh;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    add_stats(ctx->stats, S);
+    return HB_OK;
+}
+
+// The work of hb_find_fetch, with the lane's lock held
+int find_fetch(hb_ctx* ctx, const hb_ovl_shape* shape, hb_overlap* out, uint32_t* score, uint32_t* n_anchors, uint32_t* covered) {
+    const OvlResult& R = ctx->ovl.res;
+    if (!shape) return fail(ctx, HB_ERR_ARG, "null pointer");
+    if (!R.valid || shape->ticket != R.shape.ticket) return fail(ctx, HB_ERR_STATE, "the shape is not the context's latest hb_find_overlaps result");
+    const size_t n = R.shape.n_overlaps;
+    if (!n) return HB_OK;
+    if (out) memcpy(out, R.ovl.data(), n * sizeof(hb_overlap));
+    if (score) memcpy(score, R.score.data(), n * 4);
+    if (n_anchors) memcpy(n_anchors, R.n_anchors.data(), n * 4);
+    if (covered) memcpy(covered, R.covered.data(), n * 4);
+    return HB_OK;
+}
+
 // ---------------------------------------------------------------------------------- read store
 // ln(k) table from the host libm — the value Rust's f64::ln returns (src/features.rs:507)
 int upload_ln_table(hb_ctx* ctx, uint32_t max_len) {
@@ -2505,6 +2867,7 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
     ctx->host_windowing = getenv("HERRO_B200_HOST_WINDOWING") != nullptr;
     if (const char* e = getenv("HERRO_B200_ARENA_ROWS")) ctx->arena_rows_per_win = (uint32_t)std::max(atoi(e), 1);
     if (const char* e = getenv("HERRO_B200_ALN_WAVE_BYTES")) ctx->aln.wave_bytes = std::max<uint64_t>(strtoull(e, nullptr, 10), 1);
+    if (const char* e = getenv("HERRO_B200_OVL_CHUNK_BASES")) ctx->ovl.chunk_bases = std::max<uint64_t>(strtoull(e, nullptr, 10), 1);
     ctx->wt.no_fuse_ln = getenv("HERRO_B200_NO_FUSE_LN") != nullptr;
     ctx->wt.no_fuse_ffn = getenv("HERRO_B200_NO_FUSE_FFN") != nullptr;
     ctx->wt.no_fuse_attn = getenv("HERRO_B200_NO_FUSE_ATTN") != nullptr;
@@ -2523,6 +2886,8 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         if (!e) e = Cn.create({&Cn.d_in, &Cn.d_out});
         if (!e) e = Fl.lane.create({&Fl.lane.d_batch, &Fl.lane.d_rows, &Fl.lane.d_fwd, &Fl.d_tab, &Fl.d_out});
         if (!e) e = ctx->aln.create({&ctx->aln.d_reads, &ctx->aln.d_wave, &ctx->aln.d_text});
+        hb_ctx::OvlLane& O = ctx->ovl;
+        if (!e) e = O.create({&O.d_treads, &O.d_qreads, &O.d_lists, &O.d_ent, &O.d_tab, &O.d_hash, &O.d_qmin, &O.d_anc, &O.d_grp, &O.d_tmp});
         if (e) { ctx->err = e; return bail(HB_ERR_CUDA); }
         Fl.hbt = HostBatch(cuda_device);
     }
@@ -2553,7 +2918,7 @@ void hb_destroy(hb_ctx* ctx) {
     ctx->cv_work.notify_all();
     for (auto& L : ctx->lanes) if (L.worker.joinable()) L.worker.join();
     cudaSetDevice(ctx->device);
-    std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane, &ctx->aln};
+    std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane, &ctx->aln, &ctx->ovl};
     for (auto& L : ctx->lanes) all.push_back(&L);
     for (LaneBase* L : all) if (L->stream) cudaStreamSynchronize(L->stream);
     for (void* p : ctx->weight_allocs) cudaFree(p);
@@ -3231,6 +3596,16 @@ int hb_align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t b
 int hb_align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8_t* cigar_text, int32_t* status, uint32_t* matches) {
     if (!ctx) return HB_ERR_ARG;
     return stage_call(ctx, ctx->aln.mu, [&] { return align_fetch(ctx, shape, out, cigar_text, status, matches); });
+}
+
+int hb_find_overlaps(hb_ctx* ctx, uint32_t n_targets, const uint32_t* target_rids, const hb_ovl_params* params, hb_ovl_shape* shape) {
+    if (!ctx) return HB_ERR_ARG;
+    return stage_call(ctx, ctx->ovl.mu, [&] { return find_overlaps(ctx, n_targets, target_rids, params, shape); });
+}
+
+int hb_find_fetch(hb_ctx* ctx, const hb_ovl_shape* shape, hb_overlap* out, uint32_t* score, uint32_t* n_anchors, uint32_t* covered) {
+    if (!ctx) return HB_ERR_ARG;
+    return stage_call(ctx, ctx->ovl.mu, [&] { return find_fetch(ctx, shape, out, score, n_anchors, covered); });
 }
 
 }  // extern "C"

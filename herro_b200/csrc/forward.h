@@ -264,4 +264,75 @@ void launch_align_fill(const AlnArgs& a, cudaStream_t st);
 void launch_align_trace(const AlnArgs& a, cudaStream_t st);
 void launch_align_text(const AlnArgs& a, cudaStream_t st);
 
+// overlap.cu: hb_find_overlaps.  A minimizer is a key (its hash h) and a value (read index in the sketched list) << 32 | i << 1 | z.
+// An anchor is a group key (query in chunk) << 33 | (target in call) << 1 | strand and a position x << 32 | y.
+constexpr uint64_t OVL_EMPTY = ~0ull;  // an empty table slot (hashes are below 2^56)
+struct OvlSketchArgs {
+    ReadStoreView rs;        // words and word_off, indexed by store read id
+    const uint32_t* rids;    // [n] the reads to sketch
+    const uint32_t* lens;    // [n]
+    uint32_t n, k, w;
+    uint64_t* count;         // count pass: [n] minimizers per read
+    const uint64_t* offset;  // write pass: [n] each read's first slot
+    uint64_t* key;
+    uint64_t* val;
+};
+struct OvlTableArgs {
+    const uint64_t* uniq;     // [n_d] the distinct hashes of the index, ascending
+    const uint32_t* occ;      // [n_d]
+    const uint32_t* occ_off;  // [n_d] each hash's first entry
+    uint32_t n_d, max_occ;
+    uint64_t* keys;           // [mask + 1], OVL_EMPTY-filled
+    uint2* vals;              // [mask + 1] (first entry, count)
+    uint64_t mask;
+    uint32_t* n_filtered;
+};
+struct OvlAnchorArgs {
+    const uint64_t* keys;         // the table
+    const uint2* vals;
+    uint64_t mask;
+    const uint64_t* ent_val;      // the index entries' values, in hash order
+    const uint32_t* target_rids;  // [n_targets]
+    const uint64_t* mkey;         // [n_min] the chunk's query minimizers
+    const uint64_t* mval;
+    uint64_t n_min;
+    const uint32_t* q_rids;       // [chunk reads]
+    const uint32_t* q_lens;
+    uint32_t k;
+    uint64_t* count;              // count pass: [n_min]
+    const uint64_t* offset;       // write pass: [n_min]
+    uint64_t* gkey;
+    uint64_t* xy;
+};
+struct OvlGroup {  // one group's chain; kept: it passes min_score and min_anchors
+    uint64_t gkey;
+    int32_t score;
+    uint32_t n_anchors, x_first, x_last, y_first, y_last, covered, kept;
+};
+struct OvlChainArgs {
+    const uint64_t* gkey;   // [n_groups] the groups, in anchor order
+    const uint32_t* gcount;
+    const uint32_t* goff;
+    uint32_t n_groups;
+    const uint64_t* xy;     // the anchors, sorted by group and (x, y)
+    int32_t* f;             // scratch per anchor: score and predecessor
+    int32_t* pred;
+    uint32_t k, min_score, min_anchors, max_gap, bandwidth, max_iter;
+    OvlGroup* out;          // [n_groups]
+    uint32_t* n_chained;
+};
+void launch_ovl_sketch(const OvlSketchArgs& a, bool write, cudaStream_t st);
+void launch_ovl_table(const OvlTableArgs& a, cudaStream_t st);
+void launch_ovl_anchors(const OvlAnchorArgs& a, bool write, cudaStream_t st);
+void launch_ovl_chain(const OvlChainArgs& a, cudaStream_t st);
+// CUB's primitives; with tmp == nullptr each only sets `bytes`
+cudaError_t ovl_exclusive_sum(void* tmp, size_t& bytes, uint64_t* d, uint64_t n, cudaStream_t st);
+cudaError_t ovl_exclusive_sum_u32(void* tmp, size_t& bytes, const uint32_t* in, uint32_t* out, uint32_t n, cudaStream_t st);
+cudaError_t ovl_sort_pairs(void* tmp, size_t& bytes, uint64_t* keys[2], uint64_t* vals[2], int& sel, uint64_t n, int end_bit,
+                           cudaStream_t st);
+cudaError_t ovl_sort_u32(void* tmp, size_t& bytes, const uint32_t* in, uint32_t* out, uint32_t n, cudaStream_t st);
+cudaError_t ovl_runs(void* tmp, size_t& bytes, const uint64_t* in, uint64_t* uniq, uint32_t* counts, uint32_t* n_runs, uint64_t n,
+                     cudaStream_t st);
+cudaError_t ovl_select_kept(void* tmp, size_t& bytes, const OvlGroup* in, OvlGroup* out, uint32_t* n_sel, uint32_t n, cudaStream_t st);
+
 }  // namespace hb

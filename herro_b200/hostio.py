@@ -571,3 +571,48 @@ def align(reads_path: str, paf_path: str, out_dir: str, device: int = 0, min_len
     return dict(fastq_load_s=t6[0], upload_s=t6[1], paf_read_s=t6[2], align_s=t6[3], write_s=t6[4], total_s=t6[5], lines=int(c7[0]),
                 skipped=int(c7[1]), aligned=int(c7[2]), band_edge=int(c7[3]), failed=int(c7[4]), cells=int(c7[5]),
                 device_ms=int(c7[6]))
+
+
+def paf_lines(R: "Reads", got: dict) -> list:
+    """`qname qlen qstart qend +/- tname tlen tstart tend covered max(tspan, qspan) 255 s1:i:<score> cm:i:<n_anchors>` per record
+    of Context.find_overlaps, as bytes lines; hbh_paf_* (`herro align`) reads them."""
+    o, ids = got["overlaps"], R.ids
+    rows = zip(o["qid"].tolist(), o["qlen"].tolist(), o["qstart"].tolist(), o["qend"].tolist(), o["strand"].tolist(),
+               o["tid"].tolist(), o["tlen"].tolist(), o["tstart"].tolist(), o["tend"].tolist(), got["covered"].tolist(),
+               got["score"].tolist(), got["n_anchors"].tolist())
+    return [b"%s\t%d\t%d\t%d\t%c\t%s\t%d\t%d\t%d\t%d\t%d\t255\ts1:i:%d\tcm:i:%d\n" % (
+        ids[q], ql, qs, qe, 45 if st else 43, ids[t], tl, ts, te, cov, max(te - ts, qe - qs), sc, na)
+        for q, ql, qs, qe, st, t, tl, ts, te, cov, sc, na in rows]
+
+
+def overlap(reads_path: str, out_path: str, device: int = 0, min_len: int = 4096, targets_per_call: int = 50_000, **params) -> dict:
+    """`herro overlap`: the reads' all-vs-all overlaps found on the device (hb_find_overlaps), written as overlap-only PAF (gzip when
+    out_path ends in .gz).  Each call takes the next `targets_per_call` loaded reads in FASTQ order as its targets and every loaded
+    read as a query.  -> the wall time of each phase and the counts."""
+    import gzip
+    import time
+    t0 = time.perf_counter()
+    R = Reads(reads_path, min_len=min_len)
+    t1 = time.perf_counter()
+    ctx = api.Context(None, device)
+    store = R.load_into(ctx, device_bytes([device]))
+    t2 = time.perf_counter()
+    find_s = write_s = device_ms = 0.0
+    n_ovl = calls = 0
+    step = max(1, targets_per_call)
+    with (gzip.open(out_path, "wb", compresslevel=1) if out_path.endswith(".gz") else open(out_path, "wb")) as f:
+        for a in range(0, R.n, step):
+            ta = time.perf_counter()
+            got = ctx.find_overlaps(np.arange(a, min(a + step, R.n), dtype=np.uint32), **params)
+            tb = time.perf_counter()
+            f.writelines(paf_lines(R, got))
+            write_s += time.perf_counter() - tb
+            find_s += tb - ta
+            device_ms += got["shape"]["ms_device"]
+            n_ovl += len(got["overlaps"])
+            calls += 1
+    ctx.close()
+    del store
+    R.close()
+    return dict(reads=R.n, calls=calls, overlaps=n_ovl, device_ms=device_ms, fastq_load_s=t1 - t0, upload_s=t2 - t1, find_s=find_s,
+                write_s=write_s, total_s=time.perf_counter() - t0)

@@ -281,6 +281,52 @@ typedef struct hb_align_shape {     /* what one hb_align_overlaps produced      
 int hb_align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band_w, hb_align_shape* shape);
 int hb_align_fetch(hb_ctx* ctx, const hb_align_shape* shape, hb_overlap* out, uint8_t* cigar_text, int32_t* status, uint32_t* matches);
 
+/* ---- all-vs-all read overlaps ----------------------------------------------------------------- */
+typedef struct hb_ovl_params {  /* 0 in any field takes its default                                                             */
+    uint32_t k;                 /* k-mer length, 12..28 (25)                                                                  */
+    uint32_t w;                 /* minimizer window, 2..32 k-mers (17)                                                        */
+    uint32_t min_score;         /* a chain's least score (2500)                                                               */
+    uint32_t min_anchors;       /* a chain's least number of anchors (3)                                                      */
+    uint32_t max_gap;           /* the largest gap between chained anchors, on either read (5000)                             */
+    uint32_t bandwidth;         /* the largest |dx - dy| between chained anchors (150)                                        */
+    uint32_t max_iter;          /* predecessors tried per anchor (5000)                                                       */
+    uint32_t top_frac_ppm;      /* the share of distinct index hashes, in parts per million, above the occurrence threshold (5000) */
+    uint32_t min_occ;           /* the occurrence threshold's floor (10)                                                      */
+} hb_ovl_params;
+
+typedef struct hb_ovl_shape {   /* what one hb_find_overlaps produced                                                         */
+    uint64_t ticket;            /* names the result for hb_find_fetch                                                         */
+    uint32_t n_targets, n_overlaps, max_occ, n_filtered_hashes;
+    uint64_t index_entries, query_minimizers, anchors, chained_groups;
+    double ms_device;           /* device time of the call's kernels and sorts                                               */
+} hb_ovl_shape;
+
+/* The overlaps `minimap2 -x ava-ont` finds between reads, by the definition of DESIGN.md §13 (minimizer sketch, an occurrence
+ * filter on the targets' index, anchors, a chaining dynamic program): each read of the store (the queries) against the n_targets
+ * reads target_rids (the call's targets, distinct).  At most one record per (target, query) pair, query != target: the better of
+ * its two strands.  hb_find_fetch copies out any subset, as often as wanted, in call-target order and then ascending qid:
+ *   out        [n_overlaps] hb_overlap without a CIGAR (cigar NULL, cigar_len 0), ready for hb_align_overlaps
+ *   score      [n_overlaps] the chain's score
+ *   n_anchors  [n_overlaps] the chain's anchors
+ *   covered    [n_overlaps] target bases covered by the chain's k-mers (PAF column 10)
+ *
+ * Errors of the call (the previous result is gone; nothing runs):
+ *   HB_ERR_ARG       a NULL pointer, n_targets == 0, or a parameter out of range
+ *   HB_ERR_INPUT     a target rid out of range or repeated
+ *   HB_ERR_STATE     no reads yet (hb_upload_reads / hb_attach_read_store); for fetch, a shape whose ticket is not the latest result
+ *   HB_ERR_CAPACITY  a region cannot grow (the index, or the anchors of one query read)
+ *   HB_ERR_CUDA      a CUDA failure
+ *
+ * Synchronous.  The queries run in chunks of reads in rid order; a chunk's anchors take at most half of the device memory that is
+ * free when the call starts (the regions' own bytes count as free), and the regions stay allocated until the context is destroyed.
+ * With a host read store the targets and each chunk are gathered as a launch gathers its reads.  Works on an HB_FLAG_NO_MODEL
+ * context.  Calls of hb_find_overlaps / hb_find_fetch serialise among themselves on a lane of their own; they may run beside
+ * hb_submit_*, hb_flush, hb_poll_corrected and the other single-stage calls (not beside hb_upload_reads).
+ *
+ * Counters: adds to kernel_launches, h2d_bytes, d2h_bytes and host_allocs when scratch grows; the rest is in the shape. */
+int hb_find_overlaps(hb_ctx* ctx, uint32_t n_targets, const uint32_t* target_rids, const hb_ovl_params* params, hb_ovl_shape* shape);
+int hb_find_fetch(hb_ctx* ctx, const hb_ovl_shape* shape, hb_overlap* out, uint32_t* score, uint32_t* n_anchors, uint32_t* covered);
+
 /* ---- the model call alone ---------------------------------------------------------------- */
 #define HB_FWD_DEVICE_PTRS 1u  /* bases, quals and both outputs are device pointers on the context's device */
 /* The replacement of inference() (src/inference.rs:147-175) on one collated batch, for a host that keeps its own features stage,
