@@ -215,6 +215,14 @@ struct GatherSizes {  // host store: the arrays k_reads_in fills in a launch's b
     uint64_t words = 0, qual = 0;
 };
 
+// Host store: the read list of the gather being staged (list_reads), and a stamp per read that marks it listed.  One per lane kind
+// that gathers; hb_create pins every list for the context's device.
+struct ReadList {
+    PinVec<ReadCopy> list;
+    std::vector<uint32_t> stamp;
+    uint32_t gen = 0;
+};
+
 struct LastLaunch {  // host copies of per-window metadata of the most recent launch (debug taps / replay)
     bool valid = false;
     std::vector<DevWin> win;
@@ -316,10 +324,7 @@ struct hb_ctx {
         uint64_t seen_sizes = 0;  // version of hb_ctx::lane_sizes this lane has been pre-sized to
         LastLaunch last;
         std::thread worker;
-        // host store: the read list of the launch being staged, and a stamp per read that marks it listed
-        PinVec<ReadCopy> read_list;
-        std::vector<uint32_t> stamp;
-        uint32_t stamp_gen = 0;
+        ReadList reads;  // host store: the launch's reads
     };
     // Largest region capacities (and row arena) any lane has needed so far.  A lane that has not run yet (or ran smaller batches)
     // grows its regions to these while it is idle, so that its first real batch allocates nothing (r01: 26 allocations / 226 ms
@@ -369,9 +374,7 @@ struct hb_ctx {
         std::mutex mu;
         DevBuf d_reads, d_wave, d_text;
         PinBuf pin_jobs, pin_out;  // a wave's jobs and text offsets; its outputs
-        PinVec<ReadCopy> read_list;  // host store: the call's distinct reads, stamped as list_reads does for a launch lane
-        std::vector<uint32_t> stamp;
-        uint32_t stamp_gen = 0;
+        ReadList reads;            // host store: the call's reads
         AlnResult res;
         uint64_t ticket = 0;
         uint64_t wave_bytes = 8ull << 30;  // traceback bytes and op slots of one wave; HERRO_B200_ALN_WAVE_BYTES: tests shrink it to
@@ -383,10 +386,8 @@ struct hb_ctx {
     struct OvlLane : LaneBase {
         std::mutex mu;
         DevBuf d_treads, d_qreads, d_lists, d_ent, d_tab, d_hash, d_qmin, d_anc, d_grp, d_tmp;
-        PinBuf pin;  // small copies out: counts, the chosen quantile, the kept groups
-        PinVec<ReadCopy> read_list;
-        std::vector<uint32_t> stamp;
-        uint32_t stamp_gen = 0;
+        PinBuf pin;     // small copies out: counts, the chosen quantile, the kept groups
+        ReadList reads;  // host store: the targets' or a query chunk's reads
         OvlResult res;
         uint64_t ticket = 0;
         uint64_t chunk_bases = ~0ull;  // query bases per chunk at most; HERRO_B200_OVL_CHUNK_BASES: tests shrink it to run many chunks
@@ -711,6 +712,20 @@ struct Carve {
     template <class T> void operator()(T*& p, size_t n) { p = (T*)(base + bytes); bytes += al256(n * sizeof(T)); }
 };
 
+// Lay out `lay` (a callable on Carve&) in region `r`: a dry run sizes the layout, `r` grows to hold it (at least `min_bytes`, with
+// `headroom` as grow takes it), and the layout is carved again from the region.  The layout's bytes go to *bytes.
+template <class Region, class Layout>
+cudaError_t carve_region(Region& r, Layout lay, size_t* bytes = nullptr, size_t min_bytes = 0, bool headroom = true) {
+    Carve c{nullptr};
+    lay(c);
+    if (bytes) *bytes = c.bytes;
+    const cudaError_t e = r.grow(std::max(c.bytes, min_bytes), headroom);
+    if (e != cudaSuccess) return e;
+    Carve d{r.template as<uint8_t>()};
+    lay(d);
+    return cudaSuccess;
+}
+
 // A host store's gathered reads: the read list, the padded words and qualities and the offset tables, which become `rs`
 void carve_gather(Carve& c, const GatherSizes& gs, ReadsInArgs& g, ReadStoreView& rs) {
     c(g.list, gs.n_list);
@@ -730,11 +745,10 @@ void carve_gather(Carve& c, const GatherSizes& gs, ReadsInArgs& g, ReadStoreView
 // Batch region, sized from the HostBatch when a launch starts (the view's n_tgt / n_win / n_ovl / n_ow and W, and the CIGAR
 // bytes and op slots): inputs, raw and tokenised ops, everything per overlap-window, overlap, window and target, counters.  With a
 // host store also the launch's gathered reads, their read list and the offset tables, which become the view's read store.
-size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t raw_slots, const GatherSizes& gs, ReadsInArgs& g,
-                   uint8_t* base) {
+void carve_batch(Carve& c, BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t raw_slots, const GatherSizes& gs,
+                 ReadsInArgs& g) {
     const size_t nt = b.n_tgt, nw = b.n_win, no1 = std::max<size_t>(b.n_ovl, 1), ow1 = std::max<size_t>(b.n_ow, 1);
     const size_t ops = std::max<uint64_t>(op_slots, 1), raw = std::max<uint64_t>(raw_slots, 1);
-    Carve c{base};
     c(b.tgt, nt);
     c(b.win, nw);
     c(b.ovl, no1);
@@ -777,42 +791,36 @@ size_t carve_batch(BatchView& b, size_t cig_bytes, uint64_t op_slots, uint64_t r
     c(b.tgt_err, nt);
     c(b.counters, CNT_N);
     if (gs.n_reads) carve_gather(c, gs, g, b.rs);
-    return c.bytes;
 }
 
 // Row region, sized from the row arena (the view's rows_cap)
-size_t carve_rows(BatchView& b, uint8_t* base) {
+void carve_rows(Carve& c, BatchView& b) {
     const size_t rows = b.rows_cap;
-    Carve c{base};
     c(b.mat_bases, rows * ROW_BYTES);
     c(b.mat_quals, rows * ROW_BYTES);
     c(b.row_emit, rows);
     c(b.sup_row, rows);
     c(b.sup_pk, rows);
     c(b.out_bytes, rows);
-    return c.bytes;
 }
 
 // Forward region, sized from the supported positions once the first wait has counted them: the work list, the logits and
 // the workspace of one forward pass.  A pass holds whole windows (launch_tail), so it is sized for chunk_pos positions or
 // the largest window, whichever is larger.
-size_t carve_fwd(const hb_ctx* ctx, BatchView& b, FwdBufs& f, uint64_t n_sup, uint32_t max_nsup, uint8_t* base) {
+void carve_fwd(Carve& c, const hb_ctx* ctx, BatchView& b, FwdBufs& f, uint64_t n_sup, uint32_t max_nsup) {
     const size_t n = std::max<uint64_t>(n_sup, 1);
-    Carve c{base};
     c(b.fwd_win, n);
     c(b.fwd_row, n);
     c(f.logits, n * 5);
     c(f.info, n);
     c(f.ws, fwd_workspace_bytes(ctx->wt, (uint32_t)std::min<uint64_t>(std::max(ctx->chunk_pos, max_nsup), n)));
-    return c.bytes;
 }
 
 // Pinned readback of a launch: counters, then per window and per target what the per-read reassembly needs
 struct Readback {
     uint32_t *cnt, *outlen, *nsel, *L, *nsup, *terr, *sel;
 };
-size_t carve_readback(Readback& h, size_t nt, size_t nw, uint8_t* base) {
-    Carve c{base};
+void carve_readback(Carve& c, Readback& h, size_t nt, size_t nw) {
     c(h.cnt, CNT_N);
     c(h.outlen, nw);
     c(h.nsel, nw);
@@ -820,7 +828,6 @@ size_t carve_readback(Readback& h, size_t nt, size_t nw, uint8_t* base) {
     c(h.nsup, nw);
     c(h.terr, nt);
     c(h.sel, nw * TOP_K);
-    return c.bytes;
 }
 
 // The counts of a launch and the context's read store (with a host store, carve_batch points it at the gathered reads); the scratch
@@ -841,16 +848,12 @@ BatchView make_view(hb_ctx* ctx, const HostBatch& hbt) {
     return b;
 }
 
-// Point the view at a row arena of at least `rows` rows, growing the row region if needed.  Its contents are not kept: every
-// attempt of a launch fills the row region anew.
+// Point the view at a row arena of at least `rows` rows, growing the row region if needed (a region that holds rows_cap rows
+// does not grow).  Its contents are not kept: every attempt of a launch fills the row region anew.
 int set_rows(hb_ctx* ctx, hb_ctx::Lane* L, BatchView& b, uint64_t rows) {
-    if (rows > L->rows_cap) {
-        b.rows_cap = rows;
-        CK(L->d_rows.grow(carve_rows(b, nullptr)));
-        L->rows_cap = rows;
-    }
-    b.rows_cap = L->rows_cap;
-    carve_rows(b, L->d_rows.as<uint8_t>());
+    b.rows_cap = std::max(L->rows_cap, rows);
+    CK(carve_region(L->d_rows, [&](Carve& c) { carve_rows(c, b); }));
+    L->rows_cap = b.rows_cap;
     return HB_OK;
 }
 
@@ -945,15 +948,16 @@ uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
 
 // Host store: the distinct reads among the read ids that `each(add)` passes to `add` (at most `n_ids` of them), each listed once
-// in `list` with its place in the store and in the gathered region, reads laid out in order of first appearance.  `stamp` /
-// `stamp_gen` belong to the caller's lane and mark the reads listed so far.
+// in `rl.list` with its place in the store and in the gathered region, reads laid out in order of first appearance; `gs` sizes the
+// gather and `g` reads from the store.  `rl` belongs to the caller's lane.
 template <class Each>
-int list_reads(hb_ctx* ctx, PinVec<ReadCopy>& list, std::vector<uint32_t>& stamp, uint32_t& stamp_gen, size_t n_ids, Each each,
-               GatherSizes& gs) {
+int list_reads(hb_ctx* ctx, ReadList& rl, size_t n_ids, Each each, GatherSizes& gs, ReadsInArgs& g) {
     const hb_read_store* st = ctx->store;
-    if (stamp.size() != st->n_reads) { stamp.assign(st->n_reads, 0); stamp_gen = 0; }
-    if (++stamp_gen == 0) { std::fill(stamp.begin(), stamp.end(), 0u); stamp_gen = 1; }
-    const uint32_t gen = stamp_gen;
+    PinVec<ReadCopy>& list = rl.list;
+    std::vector<uint32_t>& stamp = rl.stamp;
+    if (stamp.size() != st->n_reads) { stamp.assign(st->n_reads, 0); rl.gen = 0; }
+    if (++rl.gen == 0) { std::fill(stamp.begin(), stamp.end(), 0u); rl.gen = 1; }
+    const uint32_t gen = rl.gen;
     list.clear();
     if (!list.reserve(std::min<size_t>(n_ids, st->n_reads)))
         return fail(ctx, HB_ERR_CAPACITY, "out of pinned host memory (read list)");
@@ -968,7 +972,34 @@ int list_reads(hb_ctx* ctx, PinVec<ReadCopy>& list, std::vector<uint32_t>& stamp
     };
     each(add);
     gs = GatherSizes{st->n_reads, (uint32_t)list.size(), dw, dq};
+    g.src_words = ctx->store_words;
+    g.src_qual = ctx->store_qual;
     return HB_OK;
+}
+
+// Host store: start the gather that list_reads sized and carve_gather placed, on `st`: the read list to the device, then
+// k_reads_in.  Adds its launches to `launches` and its bytes to S.h2d_bytes.
+int issue_gather(hb_ctx* ctx, const ReadList& rl, const GatherSizes& gs, const ReadsInArgs& g, cudaStream_t st, KTimer& kt,
+                 uint64_t& launches, hb_stats& S) {
+    CK(cudaMemcpyAsync((void*)g.list, rl.list.data(), vbytes(rl.list), cudaMemcpyHostToDevice, st));
+    launches += launch_reads_in(g, st, kt);
+    S.h2d_bytes += vbytes(rl.list) + gs.words * 8 + gs.qual;
+    return HB_OK;
+}
+
+// The reads that `each(add)` passes to `add` (at most `n_ids`) as a store view `rs` for work on lane L: the uploaded store, or with
+// a host store the reads gathered into `region`.  The gather's time is part of the caller's, not of a kernel class of hb_stats.
+template <class Each>
+int gather_reads(hb_ctx* ctx, LaneBase& L, ReadList& rl, DevBuf& region, size_t n_ids, Each each, ReadStoreView& rs, hb_stats& S) {
+    rs = ctx->rs;
+    if (!ctx->store) return HB_OK;
+    GatherSizes gs;
+    ReadsInArgs g{};
+    const int rc = list_reads(ctx, rl, n_ids, each, gs, g);
+    if (rc) return rc;
+    CK(carve_region(region, [&](Carve& c) { carve_gather(c, gs, g, rs); }));
+    KTimer kt;
+    return issue_gather(ctx, rl, gs, g, L.stream, kt, S.kernel_launches, S);
 }
 
 // The front half of a launch, shared by run_batch and hb_features_batch: carve the batch region for the staged batch, copy it in,
@@ -986,17 +1017,14 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
     gs = GatherSizes{};
     g = ReadsInArgs{};
     if (ctx->store) {
-        const int rc = list_reads(ctx, L->read_list, L->stamp, L->stamp_gen, hbt.tgt.size() + hbt.ovl.size(), [&](auto& add) {
+        const int rc = list_reads(ctx, L->reads, hbt.tgt.size() + hbt.ovl.size(), [&](auto& add) {
             for (const DevTarget& t : hbt.tgt) add(t.rid);
             for (const DevOverlap& o : hbt.ovl) add(o.qid);
-        }, gs);
+        }, gs, g);
         if (rc) return rc;
-        g.src_words = ctx->store_words;
-        g.src_qual = ctx->store_qual;
     }
     b = make_view(ctx, hbt);
-    CK(L->d_batch.grow(carve_batch(b, cig_bytes, op_slots, raw_slots, gs, g, nullptr)));
-    carve_batch(b, cig_bytes, op_slots, raw_slots, gs, g, L->d_batch.as<uint8_t>());
+    CK(carve_region(L->d_batch, [&](Carve& c) { carve_batch(c, b, cig_bytes, op_slots, raw_slots, gs, g); }));
     // ---- H2D straight from the pinned staging arrays of the batch
     const size_t sz[5] = {vbytes(hbt.tgt), vbytes(hbt.win), vbytes(hbt.ovl), vbytes(hbt.ow), hbt.cig.size()};
     const void* src[5] = {hbt.tgt.data(), hbt.win.data(), hbt.ovl.data(), hbt.ow.data(), hbt.cig.data()};
@@ -1009,8 +1037,7 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
     const uint64_t per_win = ctx->arena_rows_per_win ? ctx->arena_rows_per_win : (uint64_t)W + W / 2;
     int rc = set_rows(ctx, L, b, L->rows_cap ? L->rows_cap : (uint64_t)nw * per_win + 64);
     if (rc) return rc;
-    CK(L->pin_small.grow(carve_readback(h, nt, nw, nullptr)));
-    carve_readback(h, nt, nw, L->pin_small.as<uint8_t>());
+    CK(carve_region(L->pin_small, [&](Carve& c) { carve_readback(c, h, nt, nw); }));
     PHASE(0);
     L->kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
     L->kt.st = L->stream;
@@ -1020,9 +1047,8 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
         if (rc) return rc;
         CK(cudaEventRecord(L->ev[0], L->stream));
         if (gs.n_reads && attempt == 0) {  // a regrown row arena leaves the batch region, and the gathered reads, as they are
-            CK(cudaMemcpyAsync((void*)g.list, L->read_list.data(), vbytes(L->read_list), cudaMemcpyHostToDevice, L->stream));
-            *launches += launch_reads_in(g, L->stream, L->kt);
-            S.h2d_bytes += vbytes(L->read_list) + gs.words * 8 + gs.qual;
+            rc = issue_gather(ctx, L->reads, gs, g, L->stream, L->kt, *launches, S);
+            if (rc) return rc;
         }
         *launches += launch_features_a(b, L->stream, L->kt);
         CK(cudaEventRecord(L->ev[1], L->stream));
@@ -1066,8 +1092,7 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
     const uint64_t n_sup = (uint64_t)h.cnt[CNT_NSUP] | ((uint64_t)h.cnt[CNT_NSUP + 1] << 32);
     const uint32_t max_nsup = nw ? *std::max_element(h.nsup, h.nsup + nw) : 0;
     FwdBufs f;
-    CK(L->d_fwd.grow(carve_fwd(ctx, b, f, n_sup, max_nsup, nullptr)));
-    carve_fwd(ctx, b, f, n_sup, max_nsup, L->d_fwd.as<uint8_t>());
+    CK(carve_region(L->d_fwd, [&](Carve& c) { carve_fwd(c, ctx, b, f, n_sup, max_nsup); }));
     CK(cudaEventRecord(L->ev[3], L->stream));
     rc = launch_tail(ctx, L, b, f, h.nsup, nw, &launches);
     if (rc) return rc;
@@ -1295,10 +1320,11 @@ void presize_lane(hb_ctx* ctx, hb_ctx::Lane* L, const hb_ctx::LaneSizes& T) {
     cudaStreamSynchronize(L->stream);
     LastLaunch& ll = L->last;
     if (ll.valid) {  // the regions moved with their contents: carving the kept view's counts again gives the same offsets
-        carve_batch(ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, ll.gs, ll.gather, L->d_batch.as<uint8_t>());
-        carve_rows(ll.view, L->d_rows.as<uint8_t>());
+        Carve cb{L->d_batch.as<uint8_t>()}, cr{L->d_rows.as<uint8_t>()}, cf{L->d_fwd.as<uint8_t>()};
+        carve_batch(cb, ll.view, ll.cig_bytes, ll.op_slots, ll.raw_slots, ll.gs, ll.gather);
+        carve_rows(cr, ll.view);
         const uint32_t max_nsup = ll.w_nsup.empty() ? 0 : *std::max_element(ll.w_nsup.begin(), ll.w_nsup.end());
-        carve_fwd(ctx, ll.view, ll.fwd, ll.n_sup, max_nsup, L->d_fwd.as<uint8_t>());
+        carve_fwd(cf, ctx, ll.view, ll.fwd, ll.n_sup, max_nsup);
     }
 }
 
@@ -1577,8 +1603,7 @@ struct FwdIn {
     uint64_t *rowbase, *supbase;
     unsigned long long* bad;
 };
-size_t carve_fwd_in(FwdIn& a, size_t in_bytes, size_t nb, uint8_t* base) {
-    Carve c{base};
+void carve_fwd_in(Carve& c, FwdIn& a, size_t in_bytes, size_t nb) {
     c(a.tok, in_bytes);
     c(a.qual, in_bytes);
     c(a.L, nb);
@@ -1587,7 +1612,6 @@ size_t carve_fwd_in(FwdIn& a, size_t in_bytes, size_t nb, uint8_t* base) {
     c(a.rowbase, nb);
     c(a.supbase, nb);
     c(a.bad, 1);
-    return c.bytes;
 }
 
 // Where a caller's pointer lives: 1 device memory of `device` (or managed), -1 another device's memory, 0 host memory
@@ -1652,13 +1676,10 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     // ---- scratch (grow-only) and the view
     const size_t in_bytes = dev ? 0 : (size_t)rows * R_COLS;
     FwdIn hp, dp;
-    const size_t in_sz = carve_fwd_in(hp, in_bytes, B, nullptr);
-    CK(F.pin_in.grow(in_sz + 2 * al256(n * 4)));
-    carve_fwd_in(hp, in_bytes, B, F.pin_in.as<uint8_t>());
-    uint32_t* h_win = (uint32_t*)(F.pin_in.as<uint8_t>() + in_sz);
-    uint32_t* h_row = (uint32_t*)((uint8_t*)h_win + al256(n * 4));
-    CK(F.d_in.grow(in_sz));
-    carve_fwd_in(dp, in_bytes, B, F.d_in.as<uint8_t>());
+    uint32_t *h_win, *h_row;  // the work list, staged after the input region
+    size_t in_sz = 0;
+    CK(carve_region(F.pin_in, [&](Carve& c) { carve_fwd_in(c, hp, in_bytes, B); c(h_win, n); c(h_row, n); }));
+    CK(carve_region(F.d_in, [&](Carve& c) { carve_fwd_in(c, dp, in_bytes, B); }, &in_sz));
     BatchView b{};
     b.n_win = B;
     b.w_L = b.w_reflmax = dp.L;  // every window is Lmax rows long, and so is its batch
@@ -1670,8 +1691,7 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     b.mat_bases = F.d_mat.as<uint8_t>();
     b.mat_quals = b.mat_bases + al256(rows * ROW_BYTES);
     FwdBufs f;
-    CK(F.d_fwd.grow(carve_fwd(ctx, b, f, n, max_len, nullptr)));
-    carve_fwd(ctx, b, f, n, max_len, F.d_fwd.as<uint8_t>());
+    CK(carve_region(F.d_fwd, [&](Carve& c) { carve_fwd(c, ctx, b, f, n, max_len); }));
     float *h_info = nullptr, *h_logits = nullptr;
     if (!dev) {
         CK(F.pin_out.grow(al256(n * 4) + n * 20));
@@ -1761,8 +1781,7 @@ struct ConsIn {
     uint64_t *rowbase, *keybase;
     unsigned long long* bad;
 };
-size_t carve_cons_in(ConsIn& a, size_t tok_bytes, size_t logit_rows, size_t n_keys, size_t nw, uint8_t* base) {
-    Carve c{base};
+void carve_cons_in(Carve& c, ConsIn& a, size_t tok_bytes, size_t logit_rows, size_t n_keys, size_t nw) {
     c(a.tok, tok_bytes);
     c(a.logits, logit_rows * 5);
     c(a.keys, std::max<size_t>(n_keys, 1));
@@ -1772,17 +1791,14 @@ size_t carve_cons_in(ConsIn& a, size_t tok_bytes, size_t logit_rows, size_t n_ke
     c(a.rowbase, nw);
     c(a.keybase, nw);
     c(a.bad, 1);
-    return c.bytes;
 }
 // The consensus region: the rows' emit bytes and the pipeline's consensus arrays (k_cons_count, the scan, k_cons_write)
-size_t carve_cons_out(BatchView& b, size_t rows, size_t nw, uint8_t* base) {
-    Carve c{base};
+void carve_cons_out(Carve& c, BatchView& b, size_t rows, size_t nw) {
     c(b.row_emit, std::max<size_t>(rows, 1));
     c(b.out_bytes, std::max<size_t>(rows, 1));
     c(b.w_outlen, nw);
     c(b.w_outoff, nw);
     c(b.counters, CNT_N);
-    return c.bytes;
 }
 
 // The work of hb_consensus_batch, with the lane's lock held and the context's device current
@@ -1822,18 +1838,15 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
     // ---- scratch (grow-only)
     const size_t tok_bytes = dev ? 0 : (size_t)n_rows * R_COLS, logit_rows = dev ? 0 : (size_t)n_pos;
     ConsIn hp, dp;
-    const size_t in_sz = carve_cons_in(hp, tok_bytes, logit_rows, n_pos, nw, nullptr);
-    CK(Cn.pin_in.grow(in_sz));
-    carve_cons_in(hp, tok_bytes, logit_rows, n_pos, nw, Cn.pin_in.as<uint8_t>());
-    CK(Cn.d_in.grow(in_sz));
-    carve_cons_in(dp, tok_bytes, logit_rows, n_pos, nw, Cn.d_in.as<uint8_t>());
+    size_t in_sz = 0;
+    CK(carve_region(Cn.pin_in, [&](Carve& c) { carve_cons_in(c, hp, tok_bytes, logit_rows, n_pos, nw); }, &in_sz));
+    CK(carve_region(Cn.d_in, [&](Carve& c) { carve_cons_in(c, dp, tok_bytes, logit_rows, n_pos, nw); }));
     BatchView b{};
     b.n_win = (uint32_t)nw;
     b.w_L = dp.L;
     b.w_nsel = dp.nsel;
     b.w_rowbase = dp.rowbase;
-    CK(Cn.d_out.grow(carve_cons_out(b, n_rows, nw, nullptr)));
-    carve_cons_out(b, n_rows, nw, Cn.d_out.as<uint8_t>());
+    CK(carve_region(Cn.d_out, [&](Carve& c) { carve_cons_out(c, b, n_rows, nw); }));
     const size_t out_sz = al256(nw * 4) + n_rows;
     CK(Cn.pin_out.grow(out_sz));
     uint32_t* h_outlen = Cn.pin_out.as<uint32_t>();
@@ -2101,18 +2114,11 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
         if (R.n_sup[w] || R.n_ids[w]) n_lseg++;
     }
     n_bseg = R.batch_win.size();
-    Carve ct{nullptr};
-    RowSeg *t_rows, *t_batch;
-    ListSeg* t_lists;
-    ct(t_rows, n_rseg); ct(t_batch, n_bseg); ct(t_lists, n_lseg);
-    const size_t tab_bytes = ct.bytes;
-    CK(Fl.pin_tab.grow(tab_bytes));
-    CK(Fl.d_tab.grow(tab_bytes));
-    Carve hc{Fl.pin_tab.as<uint8_t>()}, dc{Fl.d_tab.as<uint8_t>()};
     RowSeg *h_rows, *h_batch, *d_rows, *d_batch;
     ListSeg *h_lists, *d_lists;
-    hc(h_rows, n_rseg); hc(h_batch, n_bseg); hc(h_lists, n_lseg);
-    dc(d_rows, n_rseg); dc(d_batch, n_bseg); dc(d_lists, n_lseg);
+    size_t tab_bytes = 0;
+    CK(carve_region(Fl.pin_tab, [&](Carve& c) { c(h_rows, n_rseg); c(h_batch, n_bseg); c(h_lists, n_lseg); }, &tab_bytes));
+    CK(carve_region(Fl.d_tab, [&](Carve& c) { c(d_rows, n_rseg); c(d_batch, n_bseg); c(d_lists, n_lseg); }));
     {
         uint64_t orow = 0, osup = 0, oid = 0;
         size_t kr = 0, kl = 0;
@@ -2138,7 +2144,6 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     int32_t* o_idx = nullptr;
     {
         const size_t rb = want_rows ? sh.n_rows * R_COLS : 0, bb = want_batch ? sh.n_batch_rows * R_COLS : 0;
-        Carve oc{nullptr};
         uint8_t *s_b, *s_q, *s_bb, *s_bq;
         uint32_t *s_sup, *s_ids;
         int32_t* s_idx;
@@ -2147,10 +2152,7 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
             c(s_bb, dev || !out->batch_bases ? 0 : bb); c(s_bq, dev || !out->batch_quals ? 0 : bb);
             c(s_sup, out->supported ? sh.n_sup * 2 : 0); c(s_idx, out->indices ? sh.n_sup : 0); c(s_ids, out->ids ? sh.n_ids : 0);
         };
-        lay(oc);
-        CK(Fl.d_out.grow(oc.bytes));
-        Carve c{Fl.d_out.as<uint8_t>()};
-        lay(c);
+        CK(carve_region(Fl.d_out, lay));
         o_b = !out->bases || !want_rows ? nullptr : dev ? out->bases : s_b;
         o_q = !out->quals || !want_rows ? nullptr : dev ? out->quals : s_q;
         o_bb = !out->batch_bases || !want_batch ? nullptr : dev ? out->batch_bases : s_bb;
@@ -2232,15 +2234,13 @@ constexpr uint32_t ALN_DEFAULT_W = 128;
 // The wave region's bytes of one overlap: its (n + 1) x 2w traceback bytes and n + m + 1 op slots
 uint64_t aln_job_bytes(uint64_t n, uint64_t m, uint32_t w) { return al256((n + 1) * 2 * w) + al256((n + m + 1) * 4); }
 
-size_t carve_wave(AlnArgs& a, AlnJob*& jobs, uint64_t*& text_off, size_t nj, uint64_t job_bytes, uint8_t* base) {
-    Carve c{base};
+void carve_wave(Carve& c, AlnArgs& a, AlnJob*& jobs, uint64_t*& text_off, size_t nj, uint64_t job_bytes) {
     c(jobs, nj);
     c(a.out, nj);
     c(text_off, nj);
     c(a.tb, job_bytes);
     a.jobs = jobs;
     a.text_off = text_off;
-    return c.bytes;
 }
 
 // The work of hb_align_overlaps, with the lane's lock held and the context's device current
@@ -2292,24 +2292,11 @@ int align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band
     LaneBase& L = A;
     // ---- the reads: the uploaded store, or the call's reads gathered from the host store
     ReadStoreView rs = ctx->rs;
-    if (ctx->store && !order.empty()) {
-        GatherSizes gs;
-        ReadsInArgs g{};
-        int rc = list_reads(ctx, A.read_list, A.stamp, A.stamp_gen, 2 * order.size(), [&](auto& add) {
+    if (!order.empty()) {
+        const int rc = gather_reads(ctx, L, A.reads, A.d_reads, 2 * order.size(), [&](auto& add) {
             for (uint32_t i : order) { add(ovl[i].tid); add(ovl[i].qid); }
-        }, gs);
+        }, rs, S);
         if (rc) return rc;
-        g.src_words = ctx->store_words;
-        g.src_qual = ctx->store_qual;
-        Carve c{nullptr};
-        carve_gather(c, gs, g, rs);
-        CK(A.d_reads.grow(c.bytes));
-        Carve c2{A.d_reads.as<uint8_t>()};
-        carve_gather(c2, gs, g, rs);
-        CK(cudaMemcpyAsync((void*)g.list, A.read_list.data(), vbytes(A.read_list), cudaMemcpyHostToDevice, L.stream));
-        KTimer kt;  // the gather's time is part of the call's, not of a kernel class of hb_stats
-        S.kernel_launches += launch_reads_in(g, L.stream, kt);
-        S.h2d_bytes += vbytes(A.read_list) + gs.words * 8 + gs.qual;
     }
     // ---- waves: the next overlaps while their traceback bytes and op slots fit the wave region.  A wave takes at most half of
     // the device's free memory (what the region already holds counts as free), so that a call beside the pipeline leaves it room;
@@ -2334,8 +2321,7 @@ int align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band
         a.w = w;
         AlnJob* d_jobs;
         uint64_t* d_toff;
-        CK(A.d_wave.grow(carve_wave(a, d_jobs, d_toff, nj, bytes, nullptr)));
-        carve_wave(a, d_jobs, d_toff, nj, bytes, A.d_wave.as<uint8_t>());
+        CK(carve_region(A.d_wave, [&](Carve& c) { carve_wave(c, a, d_jobs, d_toff, nj, bytes); }));
         CK(A.pin_jobs.grow(nj * (sizeof(AlnJob) + 8)));
         CK(A.pin_out.grow(nj * sizeof(AlnOut)));
         AlnJob* jobs = A.pin_jobs.as<AlnJob>();
@@ -2444,30 +2430,6 @@ cudaError_t cub_call(DevBuf& tmp, F f) {
     return e;
 }
 
-// The reads `rids[0..n)` as a store view: the uploaded store, or with a host store the reads gathered into `region`
-int ovl_gather(hb_ctx* ctx, hb_ctx::OvlLane& O, DevBuf& region, const uint32_t* rids, size_t n, ReadStoreView& rs, hb_stats& S) {
-    rs = ctx->rs;
-    if (!ctx->store) return HB_OK;
-    GatherSizes gs;
-    ReadsInArgs g{};
-    const int rc = list_reads(ctx, O.read_list, O.stamp, O.stamp_gen, n, [&](auto& add) {
-        for (size_t i = 0; i < n; i++) add(rids[i]);
-    }, gs);
-    if (rc) return rc;
-    g.src_words = ctx->store_words;
-    g.src_qual = ctx->store_qual;
-    Carve c{nullptr};
-    carve_gather(c, gs, g, rs);
-    CK(region.grow(c.bytes));
-    Carve c2{region.as<uint8_t>()};
-    carve_gather(c2, gs, g, rs);
-    CK(cudaMemcpyAsync((void*)g.list, O.read_list.data(), vbytes(O.read_list), cudaMemcpyHostToDevice, O.stream));
-    KTimer kt;  // the gather's time is part of the call's, not of a kernel class of hb_stats
-    S.kernel_launches += launch_reads_in(g, O.stream, kt);
-    S.h2d_bytes += vbytes(O.read_list) + gs.words * 8 + gs.qual;
-    return HB_OK;
-}
-
 struct OvlRec {
     uint32_t tpos;
     hb_overlap o;
@@ -2527,13 +2489,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
         c(d_trids, n_t); c(d_tlens, n_t); c(d_rids, n_reads); c(d_lens, n_reads); c(d_ctr, 8);
         c(d_tcnt, (size_t)n_t + 1); c(d_qcnt, (size_t)n_reads + 1);
     };
-    {
-        Carve c{nullptr};
-        carve_lists(c);
-        CK(O.d_lists.grow(c.bytes));
-        Carve c2{O.d_lists.as<uint8_t>()};
-        carve_lists(c2);
-    }
+    CK(carve_region(O.d_lists, carve_lists));
     CK(O.pin.grow(256));
     uint64_t* pin64 = O.pin.as<uint64_t>();
     uint32_t* pin32 = O.pin.as<uint32_t>();
@@ -2546,7 +2502,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
     S.h2d_bytes += 8ull * (n_t + n_reads);
     // ---- the index: the targets' minimizers sorted by hash, the occurrence threshold, the table
     ReadStoreView trs;
-    int rc = ovl_gather(ctx, O, O.d_treads, trids, n_t, trs, S);
+    int rc = gather_reads(ctx, O, O.reads, O.d_treads, n_t, [&](auto& add) { for (uint32_t i = 0; i < n_t; i++) add(trids[i]); }, trs, S);
     if (rc) return rc;
     OvlSketchArgs sk{trs, d_trids, d_tlens, n_t, k, w, d_tcnt, d_tcnt, nullptr, nullptr};
     CK(cudaMemsetAsync(d_tcnt, 0, 8ull * (n_t + 1), st));
@@ -2557,14 +2513,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
     const uint64_t E = pin64[0];
     if (E >= (1ull << 32)) return fail(ctx, HB_ERR_CAPACITY, "the index holds 2^32 minimizers or more");
     uint64_t *ek[2], *ev[2];
-    {
-        auto carve = [&](Carve& c) { c(ek[0], E); c(ek[1], E); c(ev[0], E); c(ev[1], E); };
-        Carve c{nullptr};
-        carve(c);
-        CK(O.d_ent.grow(std::max<size_t>(c.bytes, 256)));
-        Carve c2{O.d_ent.as<uint8_t>()};
-        carve(c2);
-    }
+    CK(carve_region(O.d_ent, [&](Carve& c) { c(ek[0], E); c(ek[1], E); c(ev[0], E); c(ev[1], E); }, nullptr, 256));
     sk.key = ek[0];
     sk.val = ev[0];
     launch_ovl_sketch(sk, true, st);
@@ -2572,14 +2521,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
     if (E) CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_sort_pairs(t, b, ek, ev, esel, E, 2 * k, st); }));
     uint64_t* uniq;
     uint32_t *occ, *occ_off, *occ_sorted;
-    {
-        auto carve = [&](Carve& c) { c(uniq, E); c(occ, E); c(occ_off, E); c(occ_sorted, E); };
-        Carve c{nullptr};
-        carve(c);
-        CK(O.d_tab.grow(std::max<size_t>(c.bytes, 256)));
-        Carve c2{O.d_tab.as<uint8_t>()};
-        carve(c2);
-    }
+    CK(carve_region(O.d_tab, [&](Carve& c) { c(uniq, E); c(occ, E); c(occ_off, E); c(occ_sorted, E); }, nullptr, 256));
     if (E) CK(cub_call(O.d_tmp, [&](void* t, size_t& b) { return ovl_runs(t, b, ek[esel], uniq, occ, d_ctr, E, st); }));
     CK(cudaMemcpyAsync(pin32, d_ctr, 4, cudaMemcpyDeviceToHost, st));
     if ((rc = timed_sync())) return rc;
@@ -2596,14 +2538,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
     uint64_t tcap = 1024;
     while (tcap < 2ull * n_d) tcap <<= 1;
     OvlTableArgs ta{uniq, occ, occ_off, n_d, max_occ, nullptr, nullptr, tcap - 1, d_ctr + 1};
-    {
-        auto carve = [&](Carve& c) { c(ta.keys, tcap); c(ta.vals, tcap); };
-        Carve c{nullptr};
-        carve(c);
-        CK(O.d_hash.grow(c.bytes));
-        Carve c2{O.d_hash.as<uint8_t>()};
-        carve(c2);
-    }
+    CK(carve_region(O.d_hash, [&](Carve& c) { c(ta.keys, tcap); c(ta.vals, tcap); }));
     CK(cudaMemsetAsync(ta.keys, 0xff, tcap * 8, st));
     launch_ovl_table(ta, st);
     CK(cudaGetLastError());
@@ -2624,7 +2559,8 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
         const uint32_t nq = q1 - q0;
         CK(cudaEventRecord(O.ev[1], st));
         ReadStoreView qrs;
-        if ((rc = ovl_gather(ctx, O, O.d_qreads, h_rids.data() + q0, nq, qrs, S))) return rc;
+        if ((rc = gather_reads(ctx, O, O.reads, O.d_qreads, nq, [&](auto& add) { for (uint32_t r = q0; r < q1; r++) add(r); }, qrs, S)))
+            return rc;
         OvlSketchArgs qs{qrs, d_rids + q0, d_lens + q0, nq, k, w, d_qcnt, d_qcnt, nullptr, nullptr};
         CK(cudaMemsetAsync(d_qcnt, 0, 8ull * (nq + 1), st));
         launch_ovl_sketch(qs, false, st);
@@ -2636,12 +2572,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
                          nullptr, nullptr, nullptr, nullptr};
         {
             uint64_t *mk, *mv, *ac;
-            auto carve = [&](Carve& c) { c(mk, M); c(mv, M); c(ac, M + 1); };
-            Carve c{nullptr};
-            carve(c);
-            CK(O.d_qmin.grow(c.bytes));
-            Carve c2{O.d_qmin.as<uint8_t>()};
-            carve(c2);
+            CK(carve_region(O.d_qmin, [&](Carve& c) { c(mk, M); c(mv, M); c(ac, M + 1); }));
             qs.key = mk; qs.val = mv;
             an.mkey = mk; an.mval = mv; an.count = ac; an.offset = ac;
         }
@@ -2661,14 +2592,8 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
         uint64_t *ak[2], *axy[2], *guniq;
         int32_t *f, *pred;
         uint32_t* gcnt;
-        {
-            auto carve = [&](Carve& c) { c(ak[0], A); c(ak[1], A); c(axy[0], A); c(axy[1], A); c(f, A); c(pred, A); c(guniq, A); c(gcnt, A); };
-            Carve c{nullptr};
-            carve(c);
-            CK(O.d_anc.grow(std::max<size_t>(c.bytes, 256), false));
-            Carve c2{O.d_anc.as<uint8_t>()};
-            carve(c2);
-        }
+        auto carve_anc = [&](Carve& c) { c(ak[0], A); c(ak[1], A); c(axy[0], A); c(axy[1], A); c(f, A); c(pred, A); c(guniq, A); c(gcnt, A); };
+        CK(carve_region(O.d_anc, carve_anc, nullptr, 256, false));
         an.gkey = ak[0];
         an.xy = axy[0];
         launch_ovl_anchors(an, true, st);
@@ -2685,14 +2610,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
         const uint32_t G = pin32[0];
         uint32_t* goff;
         OvlGroup *gout, *gkept;
-        {
-            auto carve = [&](Carve& c) { c(goff, G); c(gout, G); c(gkept, G); };
-            Carve c{nullptr};
-            carve(c);
-            CK(O.d_grp.grow(std::max<size_t>(c.bytes, 256)));
-            Carve c2{O.d_grp.as<uint8_t>()};
-            carve(c2);
-        }
+        CK(carve_region(O.d_grp, [&](Carve& c) { c(goff, G); c(gout, G); c(gkept, G); }, nullptr, 256));
         CK(cudaMemsetAsync(d_ctr + 3, 0, 8, st));
         uint32_t n_kept = 0;
         if (G) {
@@ -2890,6 +2808,9 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         if (!e) e = O.create({&O.d_treads, &O.d_qreads, &O.d_lists, &O.d_ent, &O.d_tab, &O.d_hash, &O.d_qmin, &O.d_anc, &O.d_grp, &O.d_tmp});
         if (e) { ctx->err = e; return bail(HB_ERR_CUDA); }
         Fl.hbt = HostBatch(cuda_device);
+        // PinVec makes its `dev` current to grow: a read list's is the device its gathering thread already has current
+        for (auto& L : ctx->lanes) L.reads.list.dev = cuda_device;
+        Fl.lane.reads.list.dev = ctx->aln.reads.list.dev = O.reads.list.dev = cuda_device;
     }
     {   // keep freed blocks in the pool instead of returning them to the driver at every synchronisation
         cudaMemPool_t pool;
