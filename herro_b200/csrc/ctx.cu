@@ -3,6 +3,7 @@
 // (cross-read batching: the reference launches one tiny forward per read, src/features.rs:582,
 // SURVEY.md F7), drive the kernel sequence on a stream, and re-assemble per-read segments
 // the way consensus() does (src/consensus.rs:86-111,222-226).
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -56,6 +57,33 @@ struct AllocScope {
         static const bool dbg = getenv("HERRO_B200_DEBUG_ALLOC") != nullptr;
         if (dbg) fprintf(stderr, "[herro_b200 alloc] %s %.1f MB %.2f ms\n", kind, (double)bytes / 1e6, (double)ns * 1e-6);
     }
+};
+
+// Whether the primary context of `dev` exists (the driver's cuDevicePrimaryCtxGetState, found through the runtime; true when it
+// cannot be asked)
+bool primary_ctx_active(int dev) {
+    using GetState = CUresult (*)(CUdevice, unsigned int*, int*);
+    static const GetState get = [] {
+        void* p = nullptr;
+        return cudaGetDriverEntryPointByVersion("cuDevicePrimaryCtxGetState", &p, 12000, cudaEnableDefault) == cudaSuccess ? (GetState)p : nullptr;
+    }();
+    unsigned int flags = 0;
+    int active = 1;
+    if (get) get((CUdevice)dev, &flags, &active);
+    return active != 0;
+}
+
+// `dev` is the calling thread's current device while the scope lives, and the caller's device is current again when it ends, so
+// that every call returns on the device it found.  A caller's device without a primary context is left alone: making it current
+// would create that context, on a GPU the process may not otherwise use.
+struct DeviceScope {
+    int prev = -1;
+    bool ok;
+    explicit DeviceScope(int dev) {
+        if (cudaGetDevice(&prev) != cudaSuccess || prev == dev || !primary_ctx_active(prev)) prev = -1;
+        ok = cudaSetDevice(dev) == cudaSuccess;
+    }
+    ~DeviceScope() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
 struct DevBuf {
@@ -133,8 +161,7 @@ struct PinVec {
         if (ncap * sizeof(T) > ((size_t)24 << 30)) ncap = want;
         AllocScope as_("pinned(staging)", ncap * sizeof(T));
         T* np = nullptr;
-        int cur = -1;
-        if (cudaGetDevice(&cur) != cudaSuccess || cur != dev) cudaSetDevice(dev);  // growth is rare: only then touch the runtime
+        DeviceScope ds(dev);  // growth is rare: only then touch the runtime
         if (cudaHostAlloc((void**)&np, ncap * sizeof(T), cudaHostAllocPortable) != cudaSuccess) return false;
         if (n) memcpy(np, p, n * sizeof(T));
         if (p) cudaFreeHost(p);
@@ -944,6 +971,19 @@ uint64_t append_segments(const uint32_t* nsel, const uint32_t* outlen, size_t nw
     return o;
 }
 
+// A target's status from its tgt_err word, and in `msg` why it failed (left as it is for HB_OK)
+int target_status(uint32_t terr, std::string& msg) {
+    if (terr & TERR_BAD_INPUT) {
+        msg = "input the reference would panic on (malformed CIGAR / window descriptor / query coordinates)";
+        return HB_ERR_INPUT;
+    }
+    if (terr & TERR_TOO_MANY_COLS) {
+        msg = "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window";
+        return HB_ERR_CAPACITY;
+    }
+    return HB_OK;
+}
+
 #define SYNC_TIMED() do { const double t__ = now_ms(); CK(cudaStreamSynchronize(L->stream)); t_wait += now_ms() - t__; } while (0)
 #define PHASE(i) do { const double t__ = now_ms(); S.ms_worker_phase[i] += t__ - t_mark; t_mark = t__; } while (0)
 
@@ -1042,7 +1082,7 @@ int run_front(hb_ctx* ctx, hb_ctx::Lane* L, const HostBatch& hbt, BatchView& b, 
     L->kt.on = ctx->time_kernels.load(std::memory_order_relaxed);
     L->kt.st = L->stream;
     for (int attempt = 0;; attempt++) {
-        if (attempt) L->kt.discard();
+        L->kt.discard();  // what a failed launch or an overflowed attempt recorded
         rc = zero_scratch(ctx, L, b);
         if (rc) return rc;
         CK(cudaEventRecord(L->ev[0], L->stream));
@@ -1131,14 +1171,7 @@ int run_batch(hb_ctx* ctx, hb_ctx::Lane* L, HostBatch& hbt) {
         const DevTarget& tg = hbt.tgt[t];
         Result r;
         r.rid = tg.rid;
-        r.status = HB_OK;
-        if (h.terr[t] & TERR_BAD_INPUT) {
-            r.status = HB_ERR_INPUT;
-            r.msg = "input the reference would panic on (malformed CIGAR / window descriptor / query coordinates)";
-        } else if (h.terr[t] & TERR_TOO_MANY_COLS) {
-            r.status = HB_ERR_CAPACITY;
-            r.msg = "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window";
-        }
+        r.status = target_status(h.terr[t], r.msg);
         o += append_segments(h.nsel + tg.win_begin, h.outlen + tg.win_begin, tg.win_end - tg.win_begin, outb + o, r.seq, r.seg_len);
         for (uint32_t w = tg.win_begin; w < tg.win_end; w++) {
             // algorithmic bytes of the pileup build for this window (SURVEY.md §8d closed form over the
@@ -1430,6 +1463,7 @@ int prepare_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_overl
         cb += ovl[i].cigar_len;
     }
     P.rid = rid; P.n_windows = n_windows; P.len = len; P.cig_bytes = cb;
+    P.raw = false;
     P.win_begin.assign(n_windows + 1, 0);
     for (uint32_t i = 0; i < n_ow; i++) {
         if (ow[i].overlap_idx >= n_ovl || ow[i].window_idx >= n_windows) return fail(ctx, HB_ERR_ARG, "overlap_window index out of range");
@@ -1506,11 +1540,8 @@ int append_target(hb_ctx* ctx, HostBatch& hbt, const PreparedTarget& P, const hb
 int stage_target(hb_ctx* ctx, const PreparedTarget& P, const hb_overlap* ovl, uint32_t n_ovl) {
     hb_ctx::ThreadSlot* slot = my_slot(ctx);
     if (slot->batch.tgt.cap == 0) acquire_batch(ctx, slot->batch);
-    std::string local_err;
-    t_err_sink = &local_err;
     const int rc = append_target(ctx, slot->batch, P, ovl, n_ovl);
-    t_err_sink = nullptr;
-    if (rc) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = local_err; return rc; }
+    if (rc) return rc;
     // `launch_targets` is shared by the submitting threads: each stages launch_targets / n_threads targets per launch,
     // so the targets in flight (and the latency to the first launch) do not grow with the thread count
     const uint32_t lt = ctx->opt.launch_targets, ns = std::max(1u, ctx->n_slots.load(std::memory_order_relaxed));
@@ -1554,7 +1585,6 @@ int prepare_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_
             if (host_extract_windows(ovl[i], i, W, n_windows, ows) != 0)
                 return fail(ctx, HB_ERR_INPUT, "malformed alignment (CIGAR / coordinates) for target " + std::to_string(rid));
         }
-        P.raw = false;
         return prepare_target(ctx, rid, n_windows, ovl, n_ovl, ows.data(), (uint32_t)ows.size(), P);
     }
     // Device windowing (windowing_dev.cu): the host only lays out which (alignment, window) pairs exist — a function of the PAF
@@ -1592,6 +1622,22 @@ int prepare_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_
 int no_model_fail(hb_ctx* ctx) {
     std::lock_guard<std::mutex> lk(ctx->mu);
     return fail(ctx, HB_ERR_STATE, "the context was created with HB_FLAG_NO_MODEL: it has no weights to run the forward with");
+}
+
+// hb_submit_target / hb_submit_alignments: `prepare(P)`, then the staging of P.  Their messages go to a string of the calling
+// thread first and reach ctx->err under ctx->mu, since the feature threads share it.
+template <class Prepare>
+int submit(hb_ctx* ctx, const hb_overlap* ovl, uint32_t n_ovl, Prepare prepare) {
+    if (!ctx) return HB_ERR_ARG;
+    if (ctx->no_model) return no_model_fail(ctx);
+    thread_local PreparedTarget P;  // its vectors keep their capacity from target to target
+    std::string err;
+    t_err_sink = &err;
+    int rc = prepare(P);
+    if (rc == HB_OK) rc = stage_target(ctx, P, ovl, n_ovl);
+    t_err_sink = nullptr;
+    if (rc) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = err; }
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------- hb_forward_batch
@@ -1649,6 +1695,17 @@ int stage_begin(hb_ctx* ctx, LaneBase& L, bool dev, void* stream) {
         CK(cudaEventRecord(L.ev[0], (cudaStream_t)stream));
         CK(cudaStreamWaitEvent(L.stream, L.ev[0], 0));
     }
+    return HB_OK;
+}
+
+// The end of a single-stage call's work on lane L, once its stream is synchronised: the kernel timer collected into S and disarmed,
+// S merged into the context's counters, and `first_err` (the first target or overlap that failed alone) made the context's message.
+int end_stage(hb_ctx* ctx, LaneBase& L, hb_stats& S, const std::string& first_err = {}) {
+    L.kt.collect(S.ms_kernel, S.n_kernel);
+    L.kt.on = false;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    add_stats(ctx->stats, S);
+    if (!first_err.empty()) ctx->err = first_err;
     return HB_OK;
 }
 
@@ -1759,15 +1816,11 @@ int forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, 
     hb_stats S{};
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, F.ev[1], F.ev[2]));
-    kt.collect(S.ms_kernel, S.n_kernel);
-    kt.on = false;
     add_forward_flops(ctx, S, n, hp.nsup, B);
     S.ms_forward = ms;
     S.supported = n;
     S.kernel_launches = launches;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    return HB_OK;
+    return end_stage(ctx, F, S);
 }
 
 // ---------------------------------------------------------------------------------- hb_consensus_batch
@@ -1938,13 +1991,9 @@ int consensus_batch(hb_ctx* ctx, uint32_t n_reads, const uint32_t* n_windows, co
     hb_stats S{};
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, Cn.ev[1], Cn.ev[2]));
-    kt.collect(S.ms_kernel, S.n_kernel);
-    kt.on = false;
     S.ms_consensus = ms;
     S.kernel_launches = launches;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    return HB_OK;
+    return end_stage(ctx, Cn, S);
 }
 
 // ---------------------------------------------------------------------------------- hb_features_batch / hb_features_fetch
@@ -1996,7 +2045,7 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
         GatherSizes gs;
         ReadsInArgs g;
         int rc = run_front(ctx, L, hbt, b, h, &launches, &total_rows, gs, g, S, t_wait, t_mark);
-        if (rc) { L->kt.discard(); return rc; }
+        if (rc) return rc;
         CK(Fl.pin_n1.grow(nw * 4));
         uint32_t* n1 = Fl.pin_n1.as<uint32_t>();
         CK(cudaMemcpyAsync(h.L, b.w_L, nw * 4, cudaMemcpyDeviceToHost, L->stream));
@@ -2006,8 +2055,6 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
         CK(cudaStreamSynchronize(L->stream));
         CK(cudaEventElapsedTime(&ms_front, L->ev[0], L->ev[2]));
         S.d2h_bytes = CNT_N * 4 + nw * 16 + nt * 4;
-        L->kt.collect(S.ms_kernel, S.n_kernel);
-        L->kt.on = false;
     }
     // ---- the caller's tables: windows of the targets in the given order, a failed target's without content
     R.rows.clear(); R.n_alns.clear(); R.n_sup.clear(); R.n_ids.clear(); R.dev_win.clear();
@@ -2024,14 +2071,11 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
         const uint32_t w_out0 = (uint32_t)R.rows.size();
         uint32_t dw0 = ~0u;
         if (R.status[i] == HB_OK) {
-            const DevTarget& tg = hbt.tgt[t_dev++];
-            if (h.terr[t_dev - 1] & TERR_BAD_INPUT) R.status[i] = HB_ERR_INPUT;
-            else if (h.terr[t_dev - 1] & TERR_TOO_MANY_COLS) R.status[i] = HB_ERR_CAPACITY;
-            if (R.status[i] == HB_OK) dw0 = tg.win_begin;
-            else if (first_err.empty())
-                first_err = "target " + std::to_string(rids[i]) + ": " +
-                            (R.status[i] == HB_ERR_INPUT ? std::string("input the reference would panic on (malformed CIGAR / window descriptor / query coordinates)")
-                                                         : "more than " + std::to_string(MAX_COLS_HARD) + " overlap-windows in one window");
+            std::string why;
+            R.status[i] = target_status(h.terr[t_dev], why);
+            if (R.status[i] == HB_OK) dw0 = hbt.tgt[t_dev].win_begin;
+            else if (first_err.empty()) first_err = "target " + std::to_string(rids[i]) + ": " + why;
+            t_dev++;
         }
         if (R.status[i] != HB_OK) n_failed++;
         for (uint32_t k = 0; k < nwin; k++) {
@@ -2069,10 +2113,7 @@ int features_batch(hb_ctx* ctx, uint32_t n_targets, const uint32_t* rids, const 
     S.kernel_launches = launches;
     // run_front times the phases of a launch worker, which this call is not: they stay out of ms_worker_phase
     std::fill(std::begin(S.ms_worker_phase), std::end(S.ms_worker_phase), 0.0);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    if (!first_err.empty()) ctx->err = first_err;
-    return HB_OK;
+    return end_stage(ctx, *L, S, first_err);
 }
 
 // The work of hb_features_fetch, with the lane's lock held and the context's device current
@@ -2197,15 +2238,11 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
     hb_stats S{};
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, L->ev[1], L->ev[2]));
-    kt.collect(S.ms_kernel, S.n_kernel);
-    kt.on = false;
     S.ms_features = ms;
     S.kernel_launches = launches;
     S.h2d_bytes = tab_bytes;
     S.d2h_bytes = d2h;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    return HB_OK;
+    return end_stage(ctx, *L, S);
 }
 
 // The frame of a single-stage ABI call: the lane's lock `mu` held throughout, the context's device current, and the messages of
@@ -2213,19 +2250,23 @@ int features_fetch(hb_ctx* ctx, const hb_features_shape* shape, const hb_feature
 template <class Body>
 int stage_call(hb_ctx* ctx, std::mutex& mu, Body body) {
     std::lock_guard<std::mutex> lk(mu);
-    int prev = -1;
-    cudaGetDevice(&prev);
+    DeviceScope ds(ctx->device);
     std::string err;
     t_err_sink = &err;
-    int rc = cudaSetDevice(ctx->device) == cudaSuccess ? HB_OK : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
-    if (rc == HB_OK) rc = body();
+    const int rc = ds.ok ? body() : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
     t_err_sink = nullptr;
-    if (prev >= 0 && prev != ctx->device) cudaSetDevice(prev);
-    if (rc != HB_OK) {
-        std::lock_guard<std::mutex> g(ctx->mu);
-        ctx->err = err;
-    }
+    if (rc) { std::lock_guard<std::mutex> g(ctx->mu); ctx->err = err; }
     return rc;
+}
+
+// The frame of a call that needs the pipeline idle (the read store, the debug taps, replay): ctx->mu held throughout, no batch
+// queued or in a lane, and the context's device current.  The messages of `body` go straight to ctx->err, since the lock is held.
+template <class Body>
+int idle_call(hb_ctx* ctx, Body body) {
+    std::unique_lock<std::mutex> lk(ctx->mu);
+    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
+    DeviceScope ds(ctx->device);
+    return ds.ok ? body() : fail(ctx, HB_ERR_CUDA, "cudaSetDevice failed");
 }
 
 // ---------------------------------------------------------------------------------- hb_align_overlaps / hb_align_fetch
@@ -2392,10 +2433,7 @@ int align_overlaps(hb_ctx* ctx, uint32_t n, const hb_overlap* ovl, uint32_t band
     R.shape = sh;
     R.valid = true;
     *shape = sh;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    if (!first_err.empty()) ctx->err = first_err;
-    return HB_OK;
+    return end_stage(ctx, L, S, first_err);
 }
 
 // The work of hb_align_fetch, with the lane's lock held
@@ -2669,9 +2707,7 @@ int find_overlaps(hb_ctx* ctx, uint32_t n_t, const uint32_t* trids, const hb_ovl
     R.shape = sh;
     R.valid = true;
     *shape = sh;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    add_stats(ctx->stats, S);
-    return HB_OK;
+    return end_stage(ctx, O, S);
 }
 
 // The work of hb_find_fetch, with the lane's lock held
@@ -2710,6 +2746,13 @@ void detach_store(hb_ctx* ctx) {
     ctx->have_reads = false;
     for (auto& L : ctx->lanes) L.last.valid = false;
     ctx->last_lane = -1;
+}
+
+// The read store changes only while no thread has targets staged for it (lock held): `call` fails otherwise
+int refuse_pending_targets(hb_ctx* ctx, const char* call) {
+    for (auto& sl : ctx->slots)
+        if (!sl->batch.tgt.empty()) return fail(ctx, HB_ERR_STATE, std::string(call) + " with targets pending: call hb_flush first");
+    return HB_OK;
 }
 
 }  // namespace
@@ -2776,7 +2819,8 @@ int hb_create(hb_ctx** out, int cuda_device, const char* model_path, const hb_op
         return bail(HB_ERR_CUDA);
     }
     if (cuda_device < 0 || cuda_device >= ndev) { ctx->err = "cuda_device out of range"; return bail(HB_ERR_ARG); }
-    if (cudaSetDevice(cuda_device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return bail(HB_ERR_CUDA); }
+    DeviceScope ds(cuda_device);
+    if (!ds.ok) { ctx->err = "cudaSetDevice failed"; return bail(HB_ERR_CUDA); }
     if (const char* e = getenv("HERRO_B200_CHUNK_POS")) ctx->chunk_pos = (uint32_t)std::min(std::max(atoi(e), 128), 65536);
     if (const char* e = getenv("HERRO_B200_LANES")) ctx->n_lanes = std::min(std::max(atoi(e), 1), (int)hb_ctx::MAX_LANES);
     if (const char* e = getenv("HERRO_B200_MIN_LAUNCH")) ctx->min_launch = (uint32_t)std::min(std::max(atoi(e), 16), 4096);
@@ -2838,7 +2882,7 @@ void hb_destroy(hb_ctx* ctx) {
     }
     ctx->cv_work.notify_all();
     for (auto& L : ctx->lanes) if (L.worker.joinable()) L.worker.join();
-    cudaSetDevice(ctx->device);
+    DeviceScope ds(ctx->device);
     std::vector<LaneBase*> all{&ctx->fwd, &ctx->cons, &ctx->feat.lane, &ctx->aln, &ctx->ovl};
     for (auto& L : ctx->lanes) all.push_back(&L);
     for (LaneBase* L : all) if (L->stream) cudaStreamSynchronize(L->stream);
@@ -2853,73 +2897,71 @@ void hb_destroy(hb_ctx* ctx) {
 int hb_upload_reads(hb_ctx* ctx, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
                     const uint8_t* const* qual) {
     if (!ctx) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    for (auto& sl : ctx->slots)
-        if (!sl->batch.tgt.empty()) return fail(ctx, HB_ERR_STATE, "hb_upload_reads with targets pending: call hb_flush first");
-    if (!seq_words || !seq_len || !qual || n_reads == 0) return fail(ctx, HB_ERR_ARG, "null/empty read store");
-    CK(cudaSetDevice(ctx->device));
-    if (ctx->store) detach_store(ctx);
-    std::vector<uint64_t> woff(n_reads + 1, 0), qoff(n_reads + 1, 0);
-    uint32_t max_len = 0;
-    for (uint32_t i = 0; i < n_reads; i++) {
-        woff[i + 1] = woff[i] + ((uint64_t)seq_len[i] + 31) / 32;
-        qoff[i + 1] = qoff[i] + seq_len[i];
-        max_len = std::max(max_len, seq_len[i]);
-        if (!seq_words[i] || !qual[i]) return fail(ctx, HB_ERR_ARG, "null read");
-    }
-    // Padded on both sides: packed 32-base extraction may touch a few words past a read, and the pileup kernel fetches the
-    // 4 bases / 4 quality bytes of a row group as whole words that may start up to 7 bytes before a read (pileup.cu).
-    constexpr size_t FRONT_WORDS = 32, FRONT_QUAL = 256;  // keeps both bases 256-byte aligned
-    CK(ctx->d_words.grow((FRONT_WORDS + woff[n_reads] + 8) * 8));
-    CK(cudaMemset(ctx->d_words.p, 0, FRONT_WORDS * 8));
-    CK(cudaMemset(ctx->d_words.as<uint64_t>() + FRONT_WORDS + woff[n_reads], 0, 8 * 8));
-    CK(ctx->d_qual.grow(FRONT_QUAL + qoff[n_reads] + 16));
-    CK(cudaMemset(ctx->d_qual.p, 33, FRONT_QUAL));
-    CK(cudaMemset(ctx->d_qual.as<uint8_t>() + FRONT_QUAL + qoff[n_reads], 33, 16));
-    CK(ctx->d_word_off.grow((n_reads + 1) * 8));
-    CK(ctx->d_qual_off.grow((n_reads + 1) * 8));
-    CK(ctx->d_len.grow((size_t)n_reads * 4));
-    // stage in pinned chunks
-    const size_t CH = 64u << 20;
-    CK(ctx->pin_in.grow(CH));
-    uint8_t* pin = ctx->pin_in.as<uint8_t>();
-    auto copy_stream = [&](auto getp, auto getn, uint8_t* dbase) -> int {
-        size_t fill = 0, doff = 0;
+    return idle_call(ctx, [&]() -> int {
+        if (const int rc = refuse_pending_targets(ctx, "hb_upload_reads")) return rc;
+        if (!seq_words || !seq_len || !qual || n_reads == 0) return fail(ctx, HB_ERR_ARG, "null/empty read store");
+        if (ctx->store) detach_store(ctx);
+        std::vector<uint64_t> woff(n_reads + 1, 0), qoff(n_reads + 1, 0);
+        uint32_t max_len = 0;
         for (uint32_t i = 0; i < n_reads; i++) {
-            const uint8_t* src = (const uint8_t*)getp(i);
-            size_t n = getn(i), so = 0;
-            while (so < n) {
-                const size_t take = std::min(n - so, CH - fill);
-                memcpy(pin + fill, src + so, take);
-                fill += take; so += take;
-                if (fill == CH) {
-                    CK(cudaMemcpy(dbase + doff, pin, fill, cudaMemcpyHostToDevice));
-                    doff += fill; fill = 0;
+            woff[i + 1] = woff[i] + ((uint64_t)seq_len[i] + 31) / 32;
+            qoff[i + 1] = qoff[i] + seq_len[i];
+            max_len = std::max(max_len, seq_len[i]);
+            if (!seq_words[i] || !qual[i]) return fail(ctx, HB_ERR_ARG, "null read");
+        }
+        // Padded on both sides: packed 32-base extraction may touch a few words past a read, and the pileup kernel fetches the
+        // 4 bases / 4 quality bytes of a row group as whole words that may start up to 7 bytes before a read (pileup.cu).
+        constexpr size_t FRONT_WORDS = 32, FRONT_QUAL = 256;  // keeps both bases 256-byte aligned
+        CK(ctx->d_words.grow((FRONT_WORDS + woff[n_reads] + 8) * 8));
+        CK(cudaMemset(ctx->d_words.p, 0, FRONT_WORDS * 8));
+        CK(cudaMemset(ctx->d_words.as<uint64_t>() + FRONT_WORDS + woff[n_reads], 0, 8 * 8));
+        CK(ctx->d_qual.grow(FRONT_QUAL + qoff[n_reads] + 16));
+        CK(cudaMemset(ctx->d_qual.p, 33, FRONT_QUAL));
+        CK(cudaMemset(ctx->d_qual.as<uint8_t>() + FRONT_QUAL + qoff[n_reads], 33, 16));
+        CK(ctx->d_word_off.grow((n_reads + 1) * 8));
+        CK(ctx->d_qual_off.grow((n_reads + 1) * 8));
+        CK(ctx->d_len.grow((size_t)n_reads * 4));
+        // stage in pinned chunks
+        const size_t CH = 64u << 20;
+        CK(ctx->pin_in.grow(CH));
+        uint8_t* pin = ctx->pin_in.as<uint8_t>();
+        auto copy_stream = [&](auto getp, auto getn, uint8_t* dbase) -> int {
+            size_t fill = 0, doff = 0;
+            for (uint32_t i = 0; i < n_reads; i++) {
+                const uint8_t* src = (const uint8_t*)getp(i);
+                size_t n = getn(i), so = 0;
+                while (so < n) {
+                    const size_t take = std::min(n - so, CH - fill);
+                    memcpy(pin + fill, src + so, take);
+                    fill += take; so += take;
+                    if (fill == CH) {
+                        CK(cudaMemcpy(dbase + doff, pin, fill, cudaMemcpyHostToDevice));
+                        doff += fill; fill = 0;
+                    }
                 }
             }
-        }
-        if (fill) CK(cudaMemcpy(dbase + doff, pin, fill, cudaMemcpyHostToDevice));
+            if (fill) CK(cudaMemcpy(dbase + doff, pin, fill, cudaMemcpyHostToDevice));
+            return HB_OK;
+        };
+        int rc = copy_stream([&](uint32_t i) { return (const void*)seq_words[i]; },
+                             [&](uint32_t i) { return (size_t)(((uint64_t)seq_len[i] + 31) / 32 * 8); }, ctx->d_words.as<uint8_t>() + FRONT_WORDS * 8);
+        if (rc) return rc;
+        rc = copy_stream([&](uint32_t i) { return (const void*)qual[i]; }, [&](uint32_t i) { return (size_t)seq_len[i]; },
+                         ctx->d_qual.as<uint8_t>() + FRONT_QUAL);
+        if (rc) return rc;
+        CK(cudaMemcpy(ctx->d_word_off.p, woff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(ctx->d_qual_off.p, qoff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(ctx->d_len.p, seq_len, (size_t)n_reads * 4, cudaMemcpyHostToDevice));
+        rc = upload_ln_table(ctx, max_len);
+        if (rc) return rc;
+        ctx->stats.h2d_bytes += woff[n_reads] * 8 + qoff[n_reads];
+        ctx->n_reads = n_reads;
+        ctx->read_len.assign(seq_len, seq_len + n_reads);
+        ctx->rs = ReadStoreView{ctx->d_words.as<uint64_t>() + FRONT_WORDS, ctx->d_word_off.as<uint64_t>(), ctx->d_len.as<uint32_t>(),
+                                ctx->d_qual.as<uint8_t>() + FRONT_QUAL, ctx->d_qual_off.as<uint64_t>(), n_reads};
+        ctx->have_reads = true;
         return HB_OK;
-    };
-    int rc = copy_stream([&](uint32_t i) { return (const void*)seq_words[i]; },
-                         [&](uint32_t i) { return (size_t)(((uint64_t)seq_len[i] + 31) / 32 * 8); }, ctx->d_words.as<uint8_t>() + FRONT_WORDS * 8);
-    if (rc) return rc;
-    rc = copy_stream([&](uint32_t i) { return (const void*)qual[i]; }, [&](uint32_t i) { return (size_t)seq_len[i]; },
-                     ctx->d_qual.as<uint8_t>() + FRONT_QUAL);
-    if (rc) return rc;
-    CK(cudaMemcpy(ctx->d_word_off.p, woff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(ctx->d_qual_off.p, qoff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(ctx->d_len.p, seq_len, (size_t)n_reads * 4, cudaMemcpyHostToDevice));
-    rc = upload_ln_table(ctx, max_len);
-    if (rc) return rc;
-    ctx->stats.h2d_bytes += woff[n_reads] * 8 + qoff[n_reads];
-    ctx->n_reads = n_reads;
-    ctx->read_len.assign(seq_len, seq_len + n_reads);
-    ctx->rs = ReadStoreView{ctx->d_words.as<uint64_t>() + FRONT_WORDS, ctx->d_word_off.as<uint64_t>(), ctx->d_len.as<uint32_t>(),
-                            ctx->d_qual.as<uint8_t>() + FRONT_QUAL, ctx->d_qual_off.as<uint64_t>(), n_reads};
-    ctx->have_reads = true;
-    return HB_OK;
+    });
 }
 
 int hb_read_store_create(hb_read_store** out, uint32_t n_reads, const uint64_t* const* seq_words, const uint32_t* seq_len,
@@ -2982,64 +3024,42 @@ int hb_read_store_destroy(hb_read_store* store) {
 
 int hb_attach_read_store(hb_ctx* ctx, hb_read_store* store) {
     if (!ctx) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    for (auto& sl : ctx->slots)
-        if (!sl->batch.tgt.empty()) return fail(ctx, HB_ERR_STATE, "hb_attach_read_store with targets pending: call hb_flush first");
-    if (!store) return fail(ctx, HB_ERR_ARG, "null read store");
-    CK(cudaSetDevice(ctx->device));
-    void* dp = nullptr;
-    CK(cudaHostGetDevicePointer(&dp, store->block, 0));
-    if (ctx->store) detach_store(ctx);
-    // the uploaded store's HBM is what this mode gives back
-    for (DevBuf* b : {&ctx->d_words, &ctx->d_word_off, &ctx->d_qual, &ctx->d_qual_off}) b->release();
-    for (auto& L : ctx->lanes) L.last.valid = false;  // their views point into the freed store
-    ctx->last_lane = -1;
-    ctx->have_reads = false;
-    const uint32_t n = store->n_reads;
-    CK(ctx->d_len.grow((size_t)n * 4));
-    CK(cudaMemcpy(ctx->d_len.p, store->len.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-    const int rc = upload_ln_table(ctx, store->max_len);
-    if (rc) return rc;
-    ctx->stats.h2d_bytes += (uint64_t)n * 4 + (uint64_t)ctx->ln_n * 8;
-    store->attached.fetch_add(1);
-    ctx->store = store;
-    ctx->store_words = (const uint64_t*)dp;
-    ctx->store_qual = (const uint8_t*)dp + store->words_bytes;
-    ctx->n_reads = n;
-    ctx->read_len = store->len;
-    ctx->rs = ReadStoreView{nullptr, nullptr, ctx->d_len.as<uint32_t>(), nullptr, nullptr, n};
-    ctx->have_reads = true;
-    return HB_OK;
+    return idle_call(ctx, [&]() -> int {
+        if (const int rc = refuse_pending_targets(ctx, "hb_attach_read_store")) return rc;
+        if (!store) return fail(ctx, HB_ERR_ARG, "null read store");
+        void* dp = nullptr;
+        CK(cudaHostGetDevicePointer(&dp, store->block, 0));
+        if (ctx->store) detach_store(ctx);
+        // the uploaded store's HBM is what this mode gives back
+        for (DevBuf* b : {&ctx->d_words, &ctx->d_word_off, &ctx->d_qual, &ctx->d_qual_off}) b->release();
+        for (auto& L : ctx->lanes) L.last.valid = false;  // their views point into the freed store
+        ctx->last_lane = -1;
+        ctx->have_reads = false;
+        const uint32_t n = store->n_reads;
+        CK(ctx->d_len.grow((size_t)n * 4));
+        CK(cudaMemcpy(ctx->d_len.p, store->len.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+        const int rc = upload_ln_table(ctx, store->max_len);
+        if (rc) return rc;
+        ctx->stats.h2d_bytes += (uint64_t)n * 4 + (uint64_t)ctx->ln_n * 8;
+        store->attached.fetch_add(1);
+        ctx->store = store;
+        ctx->store_words = (const uint64_t*)dp;
+        ctx->store_qual = (const uint8_t*)dp + store->words_bytes;
+        ctx->n_reads = n;
+        ctx->read_len = store->len;
+        ctx->rs = ReadStoreView{nullptr, nullptr, ctx->d_len.as<uint32_t>(), nullptr, nullptr, n};
+        ctx->have_reads = true;
+        return HB_OK;
+    });
 }
 
 int hb_submit_target(hb_ctx* ctx, uint32_t rid, uint32_t n_windows, const hb_overlap* ovl, uint32_t n_ovl,
                      const hb_overlap_window* ow, uint32_t n_ow) {
-    if (!ctx) return HB_ERR_ARG;
-    if (ctx->no_model) return no_model_fail(ctx);
-    thread_local PreparedTarget P;  // its vectors keep their capacity from target to target
-    P.raw = false;
-    t_err_sink = nullptr;
-    std::string local_err;
-    {   // validation errors are written to a local string first: ctx->err is shared between feature threads
-        t_err_sink = &local_err;
-        const int rc = prepare_target(ctx, rid, n_windows, ovl, n_ovl, ow, n_ow, P);
-        t_err_sink = nullptr;
-        if (rc) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = local_err; return rc; }
-    }
-    return stage_target(ctx, P, ovl, n_ovl);
+    return submit(ctx, ovl, n_ovl, [&](PreparedTarget& P) { return prepare_target(ctx, rid, n_windows, ovl, n_ovl, ow, n_ow, P); });
 }
 
 int hb_submit_alignments(hb_ctx* ctx, uint32_t rid, const hb_overlap* ovl, uint32_t n_ovl) {
-    if (!ctx) return HB_ERR_ARG;
-    if (ctx->no_model) return no_model_fail(ctx);
-    thread_local PreparedTarget P;  // scratch reused across calls
-    std::string local_err;  // validation errors are written to a local string first: ctx->err is shared between feature threads
-    t_err_sink = &local_err;
-    const int rc = prepare_alignments(ctx, rid, ovl, n_ovl, P);
-    t_err_sink = nullptr;
-    if (rc) { std::lock_guard<std::mutex> lk(ctx->mu); ctx->err = local_err; return rc; }
-    return stage_target(ctx, P, ovl, n_ovl);
+    return submit(ctx, ovl, n_ovl, [&](PreparedTarget& P) { return prepare_alignments(ctx, rid, ovl, n_ovl, P); });
 }
 
 int hb_extract_windows(const hb_overlap* ovl, uint32_t n_ovl, uint32_t window_size, uint32_t n_windows,
@@ -3170,50 +3190,49 @@ static int find_window(hb_ctx* ctx, uint32_t rid, uint32_t wid, uint32_t* w) {
 
 int hb_debug_window_shape(hb_ctx* ctx, uint32_t rid, uint32_t wid, uint32_t* shape4) {
     if (!ctx || !shape4) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    uint32_t w;
-    int rc = find_window(ctx, rid, wid, &w);
-    if (rc) return rc;
-    const LastLaunch& last = ctx->lanes[ctx->last_lane].last;
-    shape4[0] = last.w_L[w];
-    shape4[1] = last.w_nsel[w];
-    shape4[2] = last.w_nsup[w];
-    shape4[3] = 1;
-    return HB_OK;
+    return idle_call(ctx, [&]() -> int {
+        uint32_t w;
+        int rc = find_window(ctx, rid, wid, &w);
+        if (rc) return rc;
+        const LastLaunch& last = ctx->lanes[ctx->last_lane].last;
+        shape4[0] = last.w_L[w];
+        shape4[1] = last.w_nsel[w];
+        shape4[2] = last.w_nsup[w];
+        shape4[3] = 1;
+        return HB_OK;
+    });
 }
 
 int hb_debug_dump_window(hb_ctx* ctx, uint32_t rid, uint32_t wid, uint8_t* bases, uint8_t* quals, uint32_t* supported,
                          uint32_t* sup_rows, float* info_logits, float* bases_logits) {
     if (!ctx) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    CK(cudaSetDevice(ctx->device));
-    uint32_t w;
-    int rc = find_window(ctx, rid, wid, &w);
-    if (rc) return rc;
-    hb_ctx::Lane* lane = &ctx->lanes[ctx->last_lane];
-    const LastLaunch& ll = lane->last;
-    const uint32_t L = ll.w_L[w], ns = ll.w_nsup[w];
-    const uint64_t rb = ll.w_rowbase[w], sb = ll.w_supbase[w];
-    std::vector<uint8_t> tmp((size_t)L * ROW_BYTES);
-    for (int pass = 0; pass < 2; pass++) {
-        uint8_t* dst = pass ? quals : bases;
-        if (!dst || !L) continue;
-        CK(cudaMemcpy(tmp.data(), (pass ? ll.view.mat_quals : ll.view.mat_bases) + rb * ROW_BYTES, tmp.size(), cudaMemcpyDeviceToHost));
-        for (uint32_t r = 0; r < L; r++) memcpy(dst + (size_t)r * R_COLS, tmp.data() + (size_t)r * ROW_BYTES, R_COLS);
-    }
-    if (ns) {
-        std::vector<uint32_t> t(ns);
-        if (supported) {
-            CK(cudaMemcpy(t.data(), ll.view.sup_pk + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-            for (uint32_t k = 0; k < ns; k++) { supported[2 * k] = (t[k] >> 8) & 0xffffu; supported[2 * k + 1] = t[k] & 0xffu; }
+    return idle_call(ctx, [&]() -> int {
+        uint32_t w;
+        int rc = find_window(ctx, rid, wid, &w);
+        if (rc) return rc;
+        hb_ctx::Lane* lane = &ctx->lanes[ctx->last_lane];
+        const LastLaunch& ll = lane->last;
+        const uint32_t L = ll.w_L[w], ns = ll.w_nsup[w];
+        const uint64_t rb = ll.w_rowbase[w], sb = ll.w_supbase[w];
+        std::vector<uint8_t> tmp((size_t)L * ROW_BYTES);
+        for (int pass = 0; pass < 2; pass++) {
+            uint8_t* dst = pass ? quals : bases;
+            if (!dst || !L) continue;
+            CK(cudaMemcpy(tmp.data(), (pass ? ll.view.mat_quals : ll.view.mat_bases) + rb * ROW_BYTES, tmp.size(), cudaMemcpyDeviceToHost));
+            for (uint32_t r = 0; r < L; r++) memcpy(dst + (size_t)r * R_COLS, tmp.data() + (size_t)r * ROW_BYTES, R_COLS);
         }
-        if (sup_rows) CK(cudaMemcpy(sup_rows, ll.view.sup_row + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-        if (info_logits) CK(cudaMemcpy(info_logits, ll.fwd.info + sb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-        if (bases_logits) CK(cudaMemcpy(bases_logits, ll.fwd.logits + sb * 5, (size_t)ns * 20, cudaMemcpyDeviceToHost));
-    }
-    return HB_OK;
+        if (ns) {
+            std::vector<uint32_t> t(ns);
+            if (supported) {
+                CK(cudaMemcpy(t.data(), ll.view.sup_pk + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+                for (uint32_t k = 0; k < ns; k++) { supported[2 * k] = (t[k] >> 8) & 0xffffu; supported[2 * k + 1] = t[k] & 0xffu; }
+            }
+            if (sup_rows) CK(cudaMemcpy(sup_rows, ll.view.sup_row + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+            if (info_logits) CK(cudaMemcpy(info_logits, ll.fwd.info + sb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+            if (bases_logits) CK(cudaMemcpy(bases_logits, ll.fwd.logits + sb * 5, (size_t)ns * 20, cudaMemcpyDeviceToHost));
+        }
+        return HB_OK;
+    });
 }
 
 // ---- `herro features` dump (src/features.rs:724-764,806-839) ---------------------------------------------------------
@@ -3236,78 +3255,78 @@ static bool write_npy(const std::string& path, const std::string& descr, const s
 
 int hb_dump_features(hb_ctx* ctx, uint32_t rid, const char* out_dir, const char* const* read_names) {
     if (!ctx || !out_dir || !read_names) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    CK(cudaSetDevice(ctx->device));
-    if (rid >= ctx->n_reads || !read_names[rid]) return fail(ctx, HB_ERR_ARG, "rid out of range / unnamed read");
-    uint32_t w0;
-    int rc = find_window(ctx, rid, 0, &w0);
-    if (rc) return rc;
-    hb_ctx::Lane* lane = &ctx->lanes[ctx->last_lane];
-    const LastLaunch& ll = lane->last;
-    const uint32_t W = ctx->opt.window_size, n_windows = (ctx->read_len[rid] + W - 1) / W;
-    const std::string dir = std::string(out_dir) + "/" + read_names[rid];
-    {   // create_dir_all
-        std::string acc;
-        for (size_t i = 0; i <= dir.size(); i++) {
-            if (i == dir.size() || dir[i] == '/') { if (!acc.empty()) mkdir(acc.c_str(), 0777); }
-            if (i < dir.size()) acc.push_back(dir[i]);
-        }
-    }
-    static const char ASCII[13] = "ACGT*acgt#..";  // BASES_MAP inverted (src/inference.rs:23-31)
-    std::vector<uint8_t> tb, tq, feat;
-    std::vector<uint32_t> pk, order;
-    for (uint32_t wid = 0; wid < n_windows; wid++) {
-        const uint32_t w = w0 + wid;
-        if (w >= ll.win.size() || ll.win[w].rid != rid || ll.win[w].wid != wid) return fail(ctx, HB_ERR_STATE, "target is not whole in the most recent launch");
-        const uint32_t L = ll.w_L[w], ns = ll.w_nsup[w];
-        const uint64_t rb = ll.w_rowbase[w];
-        tb.resize((size_t)L * ROW_BYTES); tq.resize((size_t)L * ROW_BYTES);
-        if (L) {
-            CK(cudaMemcpy(tb.data(), ll.view.mat_bases + rb * ROW_BYTES, tb.size(), cudaMemcpyDeviceToHost));
-            CK(cudaMemcpy(tq.data(), ll.view.mat_quals + rb * ROW_BYTES, tq.size(), cudaMemcpyDeviceToHost));
-        }
-        // features: [2, L', 31] u8 — plane 0 the ASCII bases, plane 1 the quality bytes
-        feat.resize((size_t)2 * L * R_COLS);
-        for (uint32_t r = 0; r < L; r++)
-            for (int c = 0; c < R_COLS; c++) {
-                feat[(size_t)r * R_COLS + c] = (uint8_t)ASCII[tb[(size_t)r * ROW_BYTES + c] < 12 ? tb[(size_t)r * ROW_BYTES + c] : 11];
-                feat[(size_t)L * R_COLS + (size_t)r * R_COLS + c] = tq[(size_t)r * ROW_BYTES + c];
+    return idle_call(ctx, [&]() -> int {
+        if (rid >= ctx->n_reads || !read_names[rid]) return fail(ctx, HB_ERR_ARG, "rid out of range / unnamed read");
+        uint32_t w0;
+        int rc = find_window(ctx, rid, 0, &w0);
+        if (rc) return rc;
+        hb_ctx::Lane* lane = &ctx->lanes[ctx->last_lane];
+        const LastLaunch& ll = lane->last;
+        const uint32_t W = ctx->opt.window_size, n_windows = (ctx->read_len[rid] + W - 1) / W;
+        const std::string dir = std::string(out_dir) + "/" + read_names[rid];
+        {   // create_dir_all
+            std::string acc;
+            for (size_t i = 0; i <= dir.size(); i++) {
+                if (i == dir.size() || dir[i] == '/') { if (!acc.empty()) mkdir(acc.c_str(), 0777); }
+                if (i < dir.size()) acc.push_back(dir[i]);
             }
-        const std::string base = dir + "/" + std::to_string(wid);
-        if (!write_npy(base + ".features.npy", "'|u1'", "(2, " + std::to_string(L) + ", " + std::to_string(R_COLS) + ")", feat.data(), feat.size()))
-            return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".features.npy");
-        // supported: 1-D array of SupportedPos {pos: u16, ins: u8}, packed (3 bytes per record)
-        pk.resize(ns);
-        if (ns) CK(cudaMemcpy(pk.data(), ll.view.sup_pk + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-        std::vector<uint8_t> rec((size_t)ns * 3);
-        for (uint32_t k = 0; k < ns; k++) {
-            const uint16_t pos = (uint16_t)(pk[k] >> 8);
-            memcpy(&rec[(size_t)k * 3], &pos, 2);
-            rec[(size_t)k * 3 + 2] = (uint8_t)(pk[k] & 0xffu);
         }
-        if (!write_npy(base + ".supported.npy", "[('pos', '<u2'), ('ins', '|u1')]", "(" + std::to_string(ns) + ",)", rec.data(), rec.size()))
-            return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".supported.npy");
-        // ids: the query reads of ALL surviving overlaps of the window in final rank order (src/features.rs:569)
-        uint32_t n1 = 0;
-        CK(cudaMemcpy(&n1, ll.view.w_n1 + w, 4, cudaMemcpyDeviceToHost));
-        order.resize(n1);
-        if (n1) CK(cudaMemcpy(order.data(), ll.view.rank_ow + ll.win[w].ow_begin, (size_t)n1 * 4, cudaMemcpyDeviceToHost));
-        FILE* f = fopen((base + ".ids.txt").c_str(), "wb");
-        if (!f) return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".ids.txt");
-        for (uint32_t k = 0; k < n1; k++) {
-            const uint32_t q = order[k] < ll.ow_qid.size() ? ll.ow_qid[order[k]] : 0;
-            fprintf(f, "%s\n", q < ctx->n_reads && read_names[q] ? read_names[q] : "?");
+        static const char ASCII[13] = "ACGT*acgt#..";  // BASES_MAP inverted (src/inference.rs:23-31)
+        std::vector<uint8_t> tb, tq, feat;
+        std::vector<uint32_t> pk, order;
+        for (uint32_t wid = 0; wid < n_windows; wid++) {
+            const uint32_t w = w0 + wid;
+            if (w >= ll.win.size() || ll.win[w].rid != rid || ll.win[w].wid != wid) return fail(ctx, HB_ERR_STATE, "target is not whole in the most recent launch");
+            const uint32_t L = ll.w_L[w], ns = ll.w_nsup[w];
+            const uint64_t rb = ll.w_rowbase[w];
+            tb.resize((size_t)L * ROW_BYTES); tq.resize((size_t)L * ROW_BYTES);
+            if (L) {
+                CK(cudaMemcpy(tb.data(), ll.view.mat_bases + rb * ROW_BYTES, tb.size(), cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(tq.data(), ll.view.mat_quals + rb * ROW_BYTES, tq.size(), cudaMemcpyDeviceToHost));
+            }
+            // features: [2, L', 31] u8 — plane 0 the ASCII bases, plane 1 the quality bytes
+            feat.resize((size_t)2 * L * R_COLS);
+            for (uint32_t r = 0; r < L; r++)
+                for (int c = 0; c < R_COLS; c++) {
+                    feat[(size_t)r * R_COLS + c] = (uint8_t)ASCII[tb[(size_t)r * ROW_BYTES + c] < 12 ? tb[(size_t)r * ROW_BYTES + c] : 11];
+                    feat[(size_t)L * R_COLS + (size_t)r * R_COLS + c] = tq[(size_t)r * ROW_BYTES + c];
+                }
+            const std::string base = dir + "/" + std::to_string(wid);
+            if (!write_npy(base + ".features.npy", "'|u1'", "(2, " + std::to_string(L) + ", " + std::to_string(R_COLS) + ")", feat.data(), feat.size()))
+                return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".features.npy");
+            // supported: 1-D array of SupportedPos {pos: u16, ins: u8}, packed (3 bytes per record)
+            pk.resize(ns);
+            if (ns) CK(cudaMemcpy(pk.data(), ll.view.sup_pk + rb, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+            std::vector<uint8_t> rec((size_t)ns * 3);
+            for (uint32_t k = 0; k < ns; k++) {
+                const uint16_t pos = (uint16_t)(pk[k] >> 8);
+                memcpy(&rec[(size_t)k * 3], &pos, 2);
+                rec[(size_t)k * 3 + 2] = (uint8_t)(pk[k] & 0xffu);
+            }
+            if (!write_npy(base + ".supported.npy", "[('pos', '<u2'), ('ins', '|u1')]", "(" + std::to_string(ns) + ",)", rec.data(), rec.size()))
+                return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".supported.npy");
+            // ids: the query reads of ALL surviving overlaps of the window in final rank order (src/features.rs:569)
+            uint32_t n1 = 0;
+            CK(cudaMemcpy(&n1, ll.view.w_n1 + w, 4, cudaMemcpyDeviceToHost));
+            order.resize(n1);
+            if (n1) CK(cudaMemcpy(order.data(), ll.view.rank_ow + ll.win[w].ow_begin, (size_t)n1 * 4, cudaMemcpyDeviceToHost));
+            FILE* f = fopen((base + ".ids.txt").c_str(), "wb");
+            if (!f) return fail(ctx, HB_ERR_ARG, "cannot write " + base + ".ids.txt");
+            for (uint32_t k = 0; k < n1; k++) {
+                const uint32_t q = order[k] < ll.ow_qid.size() ? ll.ow_qid[order[k]] : 0;
+                fprintf(f, "%s\n", q < ctx->n_reads && read_names[q] ? read_names[q] : "?");
+            }
+            fclose(f);
         }
-        fclose(f);
-    }
-    return HB_OK;
+        return HB_OK;
+    });
 }
 
 int hb_selftest_gemm(int cuda_device, uint32_t M, uint32_t N, uint32_t K, int act, int res, uint32_t lda_extra,
                      float* max_abs_err, float* max_abs_ref, float* ms_tc, float* ms_simt) {
     if (!max_abs_err || !max_abs_ref || M % 128 || N % 128 || K % 64 || (res && act && act != 3)) return HB_ERR_ARG;
-    if (cudaSetDevice(cuda_device) != cudaSuccess) return HB_ERR_CUDA;
+    DeviceScope ds(cuda_device);
+    if (!ds.ok) return HB_ERR_CUDA;
     const size_t lda = (size_t)K + lda_extra;
     std::vector<float> hA((size_t)M * lda), hW((size_t)N * K), hb(N), hR((size_t)M * N);
     uint64_t s = 0x9E3779B97F4A7C15ull;
@@ -3398,7 +3417,8 @@ int hb_selftest_gemm(int cuda_device, uint32_t M, uint32_t N, uint32_t K, int ac
 int hb_selftest_pos_attention(int cuda_device, const uint32_t* lens, uint32_t n_seq, uint32_t heads, uint32_t head_dim,
                               const float* qkv, float* out, float* ms) {
     if (!lens || !qkv || !out || heads == 0 || (head_dim != 32 && head_dim != 64)) return HB_ERR_ARG;
-    if (cudaSetDevice(cuda_device) != cudaSuccess) return HB_ERR_CUDA;
+    DeviceScope ds(cuda_device);
+    if (!ds.ok) return HB_ERR_CUDA;
     const size_t D = (size_t)heads * head_dim;
     std::vector<uint64_t> base(n_seq);
     uint64_t rows = 0;
@@ -3450,33 +3470,32 @@ int hb_selftest_pos_attention(int cuda_device, const uint32_t* lens, uint32_t n_
 
 int hb_replay_last_launch(hb_ctx* ctx, uint32_t iters, float* ms) {
     if (!ctx || !ms) return HB_ERR_ARG;
-    std::unique_lock<std::mutex> lk(ctx->mu);
-    ctx->cv_idle.wait(lk, [&] { return ctx->idle(); });
-    CK(cudaSetDevice(ctx->device));
-    if (ctx->last_lane < 0 || !ctx->lanes[ctx->last_lane].last.valid) return fail(ctx, HB_ERR_STATE, "no launch to replay");
-    hb_ctx::Lane* L = &ctx->lanes[ctx->last_lane];
-    const BatchView b = L->last.view;
-    uint64_t launches = 0;
-    L->kt.on = false;
-    L->kt.st = L->stream;
-    CK(cudaStreamSynchronize(L->stream));
-    CK(cudaEventRecord(L->ev[6], L->stream));
-    for (uint32_t it = 0; it < iters; it++) {
-        int rc = zero_scratch(ctx, L, b);
-        if (rc) return rc;
-        if (L->last.gs.n_reads) launches += launch_reads_in(L->last.gather, L->stream, L->kt);
-        launches += launch_features_a(b, L->stream, L->kt);
-        launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
-        launches += launch_features_c1(b, L->stream, L->kt);
-        rc = launch_tail(ctx, L, b, L->last.fwd, L->last.w_nsup.data(), L->last.w_nsup.size(), &launches);
-        if (rc) return rc;
-    }
-    CK(cudaEventRecord(L->ev[7], L->stream));
-    CK(cudaStreamSynchronize(L->stream));
-    CK(cudaEventElapsedTime(ms, L->ev[6], L->ev[7]));
-    L->kt.discard();
-    ctx->stats.kernel_launches += launches;
-    return HB_OK;
+    return idle_call(ctx, [&]() -> int {
+        if (ctx->last_lane < 0 || !ctx->lanes[ctx->last_lane].last.valid) return fail(ctx, HB_ERR_STATE, "no launch to replay");
+        hb_ctx::Lane* L = &ctx->lanes[ctx->last_lane];
+        const BatchView b = L->last.view;
+        uint64_t launches = 0;
+        L->kt.on = false;
+        L->kt.st = L->stream;
+        CK(cudaStreamSynchronize(L->stream));
+        CK(cudaEventRecord(L->ev[6], L->stream));
+        for (uint32_t it = 0; it < iters; it++) {
+            int rc = zero_scratch(ctx, L, b);
+            if (rc) return rc;
+            if (L->last.gs.n_reads) launches += launch_reads_in(L->last.gather, L->stream, L->kt);
+            launches += launch_features_a(b, L->stream, L->kt);
+            launches += launch_pileup(b, L->stream, L->kt, ctx->pileup_v1);
+            launches += launch_features_c1(b, L->stream, L->kt);
+            rc = launch_tail(ctx, L, b, L->last.fwd, L->last.w_nsup.data(), L->last.w_nsup.size(), &launches);
+            if (rc) return rc;
+        }
+        CK(cudaEventRecord(L->ev[7], L->stream));
+        CK(cudaStreamSynchronize(L->stream));
+        CK(cudaEventElapsedTime(ms, L->ev[6], L->ev[7]));
+        L->kt.discard();
+        ctx->stats.kernel_launches += launches;
+        return HB_OK;
+    });
 }
 
 int hb_forward_batch(hb_ctx* ctx, uint32_t B, uint32_t Lmax, const uint8_t* bases, const uint8_t* quals, const int32_t* lens,

@@ -19,7 +19,9 @@
  * Threading: hb_submit_* may be called concurrently from the host's feature threads
  * (`-t`, src/lib.rs:159-187); hb_poll_corrected / hb_release_result from one thread per
  * context (the former consensus thread feeding correction_writer, src/lib.rs:267-291).
- * One context per GPU (`-d`), like the reference's per-device worker group.
+ * One context per GPU (`-d`), like the reference's per-device worker group.  Every call
+ * returns with the calling thread's current CUDA device as it found it, unless that device
+ * had no primary context yet: making it current again would create one.
  */
 #ifndef HERRO_B200_H
 #define HERRO_B200_H
