@@ -17,6 +17,10 @@ PROFILES = {
     # sub, ins, del, hp_boost  (SURVEY.md §8d)
     "r10": (0.004, 0.003, 0.005, 0.6),
     "r9": (0.015, 0.015, 0.025, 0.6),
+    # low-error reads: long CIGAR ops and tied rankings.  The haplotype SNPs / indels (het_snp, het_indel) and the long
+    # deletions stay, so supported positions still appear at het sites.
+    "exact": (0.0, 0.0, 0.0, 0.0),
+    "q30": (1e-3, 1e-4, 1e-4, 0.6),
 }
 
 
